@@ -237,17 +237,21 @@ k_forest_predict_ranked(const __grid_constant__ RankedParams p) {
         int best_s = 0, cur_s = 0;
         // The leaf values of a group are only added (in tree order: bit-identical float64 sums) while
         // the NEXT group -- possibly of the next chunk -- walks its first level, so that the serial DADD
-        // chain hides behind shared-memory latency instead of idling the warp.
+        // chain hides behind shared-memory latency instead of idling the warp.  A slot with nothing to add
+        // holds -0.0: x + (-0.0) == x bit for bit for every x (also -0.0 and NaN), so the adds need no
+        // per-tree test (a test and two selects per tree were ~4 % of the group's instructions).
         double pend[kIlp];
-        int n_pend = 0;
+#pragma unroll
+        for (int j = 0; j < kIlp; ++j) pend[j] = -0.0;
         for (int c = 0; c < F.n_chunks; ++c, ++k) {
             const int b = (int)(k % kStages);
             const int s = F.chunk_seq[c];
             if (s != cur_s) {  // previous sequence is complete
 #pragma unroll
-                for (int j = 0; j < kIlp; ++j)
-                    if (j < n_pend) acc += pend[j];
-                n_pend = 0;
+                for (int j = 0; j < kIlp; ++j) {
+                    acc += pend[j];
+                    pend[j] = -0.0;
+                }
                 if (live && p.out_margin) p.out_margin[i * F.n_seq + cur_s] = acc;
                 if (cur_s == 0) { best = acc; margin0 = acc; }
                 else if (acc > best) { best = acc; best_s = cur_s; }
@@ -279,12 +283,11 @@ k_forest_predict_ranked(const __grid_constant__ RankedParams p) {
 #pragma unroll
                     for (int j = 0; j < kIlp; ++j) {
                         w[j] = step_node<kWide, T>(nodes, w[j], feat, lane_off);
-                        if (j < n_pend) acc += pend[j];
+                        acc += pend[j];
                     }
                 } else {
 #pragma unroll
-                    for (int j = 0; j < kIlp; ++j)
-                        if (j < n_pend) acc += pend[j];
+                    for (int j = 0; j < kIlp; ++j) acc += pend[j];
                 }
                 for (int d = 2; d < depth; ++d) {
 #pragma unroll
@@ -299,7 +302,11 @@ k_forest_predict_ranked(const __grid_constant__ RankedParams p) {
 #pragma unroll
                     for (int j = 0; j < kIlp; ++j) pend[j] = leaf_value(leaves, lb[j] + (int)__byte_perm(w[j], 0, 0x4421));
                 }
-                n_pend = n_trees - q < kIlp ? n_trees - q : kIlp;
+                if (q + kIlp > n_trees) {  // the surplus slots' values (tree 0 again) are not added
+#pragma unroll
+                    for (int j = 1; j < kIlp; ++j)
+                        if (q + j >= n_trees) pend[j] = -0.0;
+                }
             }
             // this warp is done with buffer b; the last warp to leave refills it with stream chunk
             // k + kStages (no producer thread, nobody polls)
@@ -317,8 +324,7 @@ k_forest_predict_ranked(const __grid_constant__ RankedParams p) {
             }
         }
 #pragma unroll
-        for (int j = 0; j < kIlp; ++j)  // the last group of the last sequence
-            if (j < n_pend) acc += pend[j];
+        for (int j = 0; j < kIlp; ++j) acc += pend[j];  // the last group of the last sequence
         if (live && p.out_margin) p.out_margin[i * F.n_seq + cur_s] = acc;
         if (cur_s == 0) { best = acc; margin0 = acc; }
         else if (acc > best) { best = acc; best_s = cur_s; }

@@ -77,3 +77,32 @@ def random_forest(n_features, n_classes, n_iter, feature_thresholds, rng, max_de
         "feature": feature, "threshold": threshold, "missing_left": missing_left, "left": left, "right": right,
         "value": value,
     }
+
+
+def mixed_depth_forest(n_features, n_classes, depth_caps, feature_thresholds, rng, leaf_scale=0.01):
+    """Random forest whose tree t (boosting order: round-major, one tree per class) is at most
+    ``depth_caps[t]`` deep (<= 31 leaves; a cap of 0 is a single leaf): forests that mix single-leaf,
+    shallow and deep trees in any pattern, for the ranked kernel's per-tree walk depth."""
+    caps = np.asarray(depth_caps, dtype=np.int64)
+    S = 1 if n_classes <= 2 else n_classes
+    assert len(caps) % S == 0
+    pool = {int(d): random_forest(n_features, 2, int((caps == d).sum()), feature_thresholds, rng, max_depth=int(d),
+                                  leaf_scale=leaf_scale)
+            for d in np.unique(caps)}
+    used = {d: 0 for d in pool}
+    keys = ("feature", "threshold", "missing_left", "left", "right", "value")
+    parts = {k: [] for k in keys}
+    sizes = []
+    for d in caps.tolist():
+        f = pool[d]
+        a, b = int(f["tree_offset"][used[d]]), int(f["tree_offset"][used[d] + 1])
+        used[d] += 1
+        for k in keys:
+            parts[k].append(f[k][a:b])
+        sizes.append(b - a)
+    tree_offset = np.zeros(len(caps) + 1, dtype=np.int64)
+    tree_offset[1:] = np.cumsum(sizes)
+    out = {k: np.concatenate(v) for k, v in parts.items()}
+    out.update({"n_features": int(n_features), "n_classes": int(n_classes), "baseline": np.zeros(S),
+                "tree_seq": (np.arange(len(caps)) % S).astype(np.int32), "tree_offset": tree_offset})
+    return out
