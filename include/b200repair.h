@@ -113,6 +113,24 @@ int dr_quartiles(dr_ctx* ctx, const double* col, int64_t n_rows, double* out_q, 
 int dr_range_flag(dr_ctx* ctx, const double* col, int64_t n_rows, double lower, double upper, uint32_t* bitmap,
                   void* stream);
 
+/* ---- a4: LOFOutlierErrorDetector --------------------------------------------------------------
+ * Replaces sklearn.neighbors.LocalOutlierFactor(novelty=False).fit_predict on one continuous column
+ * (errors.py:219-245, 302-312), computed over the sorted distinct values instead of per row.
+ * dr_lof_score: u device float64[n_entries] strictly ascending, cnt device int64[n_entries] (>= 1 each;
+ * the NULL rows already merged in as copies of the median), k in [1, 64].  Writes verdict device
+ * uint8[n_entries] (1 = outlier, lof > 1.5) and kdist / lrd device float64[n_entries] (outputs and
+ * workspace); lof device float64[n_entries] or NULL.  Equal-distance ties take the smaller value
+ * first.  Three passes, ~81 bytes per entry.
+ * dr_lof_median: entries holding ranks r0 and r1 (0-based) of the multiset given by the counts
+ * cnt device int64[n_entries]; out_entry host int64[2] (-1 = rank out of range).  Synchronises.
+ * dr_lof_flag: flags  verdict[code] != 0  for code >= 0 and  null_verdict != 0  for NULL cells. */
+int dr_lof_score(dr_ctx* ctx, const double* u, const int64_t* cnt, int64_t n_entries, int32_t k, uint8_t* verdict,
+                 double* kdist, double* lrd, double* lof, void* stream);
+int dr_lof_median(dr_ctx* ctx, const int64_t* cnt, int64_t n_entries, int64_t r0, int64_t r1, int64_t* out_entry,
+                  void* stream);
+int dr_lof_flag(dr_ctx* ctx, const int32_t* col, int64_t n_rows, const uint8_t* verdict, int32_t dict_size,
+                int32_t null_verdict, uint32_t* bitmap, void* stream);
+
 /* ---- a3: ConstraintErrorDetector --------------------------------------------------------------
  * Replaces ErrorDetectorApi.detectErrorCellsFromConstraints (ErrorDetectorApi.scala:48-58,
  * 189-244); the constraint text is parsed on the host (DenialConstraints.scala:82-225).

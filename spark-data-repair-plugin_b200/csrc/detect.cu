@@ -39,12 +39,14 @@ __device__ __forceinline__ void rows_to_bitmap(int64_t n_rows, uint32_t* __restr
     }
 }
 
+// null_hit: whether a NULL cell (code < 0) is flagged -- always for the LUT detectors, the verdict of the
+// median's entry for LOF (NULL cells are filled with the median)
 __global__ void __launch_bounds__(kThreads) k_lut_scan(const int32_t* __restrict__ col, int64_t n_rows,
-                                                       const uint8_t* __restrict__ lut, int dict_size,
+                                                       const uint8_t* __restrict__ lut, int dict_size, bool null_hit,
                                                        uint32_t* __restrict__ bm) {
     rows_to_bitmap(n_rows, bm, [&](int64_t r) {
         const int c = __ldcs(col + r);
-        return c < 0 || (c < dict_size && __ldg(lut + c) != 0);
+        return c < 0 ? null_hit : (c < dict_size && __ldg(lut + c) != 0);
     });
 }
 
@@ -303,7 +305,18 @@ int dr_lut_scan(dr_ctx* ctx, const int32_t* col, int64_t n_rows, const uint8_t* 
     DR_REQUIRE(ctx, col && bitmap && (lut || dict_size == 0), "null pointer");
     if (n_rows <= 0) return DR_OK;
     k_lut_scan<<<dr_grid_for(ctx, n_rows, kThreads, kCtasPerSm), kThreads, 0, (cudaStream_t)stream>>>(
-        col, n_rows, lut, dict_size, bitmap);
+        col, n_rows, lut, dict_size, true, bitmap);
+    DR_LAUNCHED(ctx);
+    return DR_OK;
+}
+
+int dr_lof_flag(dr_ctx* ctx, const int32_t* col, int64_t n_rows, const uint8_t* verdict, int32_t dict_size,
+                int32_t null_verdict, uint32_t* bitmap, void* stream) {
+    if (!ctx) return DR_ERR_INVALID;
+    DR_REQUIRE(ctx, col && bitmap && (verdict || dict_size == 0), "null pointer");
+    if (n_rows <= 0) return DR_OK;
+    k_lut_scan<<<dr_grid_for(ctx, n_rows, kThreads, kCtasPerSm), kThreads, 0, (cudaStream_t)stream>>>(
+        col, n_rows, verdict, dict_size, null_verdict != 0, bitmap);
     DR_LAUNCHED(ctx);
     return DR_OK;
 }

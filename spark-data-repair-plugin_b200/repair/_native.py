@@ -75,6 +75,10 @@ _SIGNATURES = {
     "dr_lut_scan": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int32, c_void_p, c_void_p]),
     "dr_quartiles": (c_int, [c_void_p, c_void_p, c_int64, POINTER(c_double), POINTER(c_int64), c_void_p]),
     "dr_range_flag": (c_int, [c_void_p, c_void_p, c_int64, c_double, c_double, c_void_p, c_void_p]),
+    "dr_lof_score": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                             c_void_p]),
+    "dr_lof_median": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, POINTER(c_int64), c_void_p]),
+    "dr_lof_flag": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int32, c_int32, c_void_p, c_void_p]),
     "dr_dc_const": (c_int, [c_void_p, _PP, POINTER(c_int32), POINTER(c_int32), c_int, c_int64, c_void_p, c_void_p]),
     "dr_dc_fd_build": (c_int, [c_void_p, _PP, POINTER(c_int64), c_int, c_void_p, c_int64, c_int64, c_void_p,
                                c_void_p, c_void_p]),
@@ -301,6 +305,23 @@ class Context:
 
     def range_flag(self, col, n_rows, lower, upper, bitmap):
         self._check(self.lib.dr_range_flag(self._h, _dp(col), n_rows, lower, upper, _dp(bitmap), self._stream()))
+
+    def lof_score(self, u, cnt, k, verdict, kdist, lrd, lof=None):
+        """LOF over sorted distinct values u (float64) with multiplicities cnt (int64), all device tensors of
+        one length; writes verdict (uint8, 1 = outlier), kdist and lrd, and lof when given."""
+        self._check(self.lib.dr_lof_score(self._h, _dp(u), _dp(cnt), int(u.numel()), int(k), _dp(verdict),
+                                          _dp(kdist), _dp(lrd), _dp(lof), self._stream()))
+
+    def lof_median(self, cnt, r0, r1):
+        """-> (entry holding rank r0, entry holding rank r1) of the multiset counted by cnt (device int64)."""
+        out = (c_int64 * 2)()
+        self._check(self.lib.dr_lof_median(self._h, _dp(cnt), int(cnt.numel()), int(r0), int(r1), out,
+                                           self._stream()))
+        return int(out[0]), int(out[1])
+
+    def lof_flag(self, col, n_rows, verdict, dict_size, null_verdict, bitmap):
+        self._check(self.lib.dr_lof_flag(self._h, _dp(col), n_rows, _dp(verdict), dict_size, int(bool(null_verdict)),
+                                         _dp(bitmap), self._stream()))
 
     def dc_const(self, cols, ops, args, n_rows, row_bitmap):
         cp, _k = _ptr_array([c.data_ptr() for c in cols])

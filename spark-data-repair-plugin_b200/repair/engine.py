@@ -288,11 +288,21 @@ class Engine:
             return self._hist_cache[attr]
         if attr in self._raw_cache:
             return self._raw_cache[attr]
+        self._raw_cache[attr] = self.raw_value_counts_dev(attr).cpu().numpy()
+        return self._raw_cache[attr]
+
+    def launch_raw_counts(self, attr):
+        """LOCAL int64[dict_size + 1] counts of the raw column (slot 0 = NULL) on the device, not exchanged."""
+        col = self.table.by_name[attr]
         hist = self.torch.zeros(col.dict_size + 1, dtype=self.torch.int64, device=self.device)
         self.ctx.scan_hist([self.dt.col(attr)], [col.dict_size], self.n_rows, [None], hist)
+        return hist
+
+    def raw_value_counts_dev(self, attr):
+        """Device-resident variant of raw_value_counts (not cached: a dictionary may have 10^8 entries)."""
+        hist = self.launch_raw_counts(attr)
         self.exchange([(hist, "sum")])
-        self._raw_cache[attr] = hist.cpu().numpy()
-        return self._raw_cache[attr]
+        return hist
 
     # ---- detectors -----------------------------------------------------------------------------
     def _or_rows_into(self, row_bitmap, attrs, bitmaps):
@@ -593,6 +603,106 @@ class Engine:
                 bitmaps[a] = self.new_bitmap()
             self.ctx.range_flag(self.dt.val(a), self.n_rows, lower, upper, bitmaps[a])
 
+    def detect_lof(self, targets, bitmaps, ex_parts=None, after=None):
+        """LOFOutlierErrorDetector: LocalOutlierFactor(novelty=False) with its defaults over every continuous
+        target, on the column's sorted dictionary (dr_lof_score; see csrc/lof.cu).  The global value counts
+        of each column join the pass's exchange (`ex_parts`); the scoring and the row flags run once they
+        are global (`after`), so every shard computes the same verdicts and flags its own rows.  Called
+        without ex_parts / after (stand-alone detector) it does both at once."""
+        now = ex_parts is None
+        if now:
+            ex_parts, after = [], []
+        for a in self.table.continuous_attrs:
+            if a not in targets:
+                continue
+            u = np.asarray(self.table.by_name[a].dictionary, dtype=np.float64)
+            if not np.isfinite(u).all():
+                raise ValueError("LOFOutlierErrorDetector: column '{}' contains infinity".format(a))
+            if a not in bitmaps:
+                bitmaps[a] = self.new_bitmap()
+            hist = self.launch_raw_counts(a)
+            ex_parts.append((hist, "sum"))
+            after.append(lambda a=a, u=u, hist=hist: self._lof_flag(a, u, hist, bitmaps))
+        if now:
+            self.exchange(ex_parts)
+            for fn in after:
+                fn()
+
+    def lof_median(self, u, hist):
+        """np.median of the non-NULL cells from the global counts (slot 0 = NULL) -> (median, #non-NULL)."""
+        n_valid = self.n_rows_global - int(hist[0].item())
+        if n_valid <= 0:
+            return None, 0
+        r0, r1 = (n_valid - 1) // 2, n_valid // 2
+        i0, i1 = self.ctx.lof_median(hist[1:], r0, r1)
+        return (float(u[i0]) if r0 == r1 else (float(u[i0]) + float(u[i1])) / 2), n_valid
+
+    def lof_entries(self, u, hist):
+        """The weighted entries LOF runs over: the dictionary with the NULL rows merged in as copies of the
+        median.  -> (device u float64[D'], device cnt int64[D'], k, entry of the median or -1, inserted)"""
+        torch = self.torch
+        n = self.n_rows_global
+        median, n_valid = self.lof_median(u, hist)
+        if n < 2 or n_valid == 0:
+            return None
+        d_u = torch.from_numpy(u).to(self.device)
+        cnt = hist[1:]
+        n_null = n - n_valid
+        entry, inserted = -1, False
+        if n_null:
+            entry = int(np.searchsorted(u, median))
+            if entry < len(u) and u[entry] == median:
+                cnt = cnt.clone()
+                cnt[entry] += n_null
+            else:
+                inserted = True
+                d_u = torch.cat([d_u[:entry], torch.tensor([median], dtype=torch.float64, device=self.device),
+                                 d_u[entry:]])
+                cnt = torch.cat([cnt[:entry], torch.tensor([n_null], dtype=torch.int64, device=self.device),
+                                 cnt[entry:]])
+        return d_u, cnt.contiguous(), max(1, min(20, n - 1)), entry, inserted
+
+    def _lof_flag(self, a, u, hist, bitmaps):
+        got = self.lof_entries(u, hist)
+        if got is None:
+            return
+        d_u, cnt, k, entry, inserted = got
+        torch = self.torch
+        n_e = int(d_u.numel())
+        verdict = torch.empty(n_e, dtype=torch.uint8, device=self.device)
+        kdist = torch.empty(n_e, dtype=torch.float64, device=self.device)
+        lrd = torch.empty(n_e, dtype=torch.float64, device=self.device)
+        self.ctx.lof_score(d_u, cnt, k, verdict, kdist, lrd)
+        del kdist, lrd
+        null_verdict = bool(verdict[entry].item()) if entry >= 0 else False
+        lut = torch.cat([verdict[:entry], verdict[entry + 1:]]) if inserted else verdict
+        self.ctx.lof_flag(self.dt.col(a), self.n_rows, lut, len(u), null_verdict, bitmaps[a])
+
+    def detect_sklearn(self, targets, bitmaps, factory):
+        """ScikitLearnBackedErrorDetector (errors.py:219-245): a user estimator's fit_predict over each
+        continuous target with its NULL cells filled with the median.  The estimator is a Python object, so
+        this is the one detector that computes on the host; the labels travel back as bitmaps."""
+        import pandas as pd
+        if self.dist is not None:
+            raise NotImplementedError("ScikitLearnBackedErrorDetector runs a host-side estimator over a whole "
+                                      "column and does not support setDistributed runs")
+        for a in self.table.continuous_attrs:
+            if a not in targets:
+                continue
+            vals = self.dt.val(a)[:self.n_rows].cpu().numpy()
+            valid = vals[~np.isnan(vals)]
+            if len(valid) == 0:
+                continue
+            filled = np.where(np.isnan(vals), np.median(valid), vals)
+            pred = np.asarray(factory().fit_predict(pd.DataFrame({a: filled})))
+            rows = np.nonzero(pred < 0)[0]
+            got = self.bitmaps_from_cells(rows, [a] * len(rows))
+            if a in got:
+                if a in bitmaps:
+                    self.ctx.bitmap_or(bitmaps[a], got[a], self.n_rows)
+                else:
+                    bitmaps[a] = got[a]
+
     def bitmaps_from_cells(self, positions, attrs):
         """User-supplied error cells (setErrorCells) -> bitmaps, built on the host."""
         out = {}
@@ -848,14 +958,14 @@ class Engine:
 
     # ---- ErrorModel.detect -----------------------------------------------------------------------
     def detect(self, detectors, targets, discrete_thres, opts, given_cells=None):
-        """detectors: list of dicts {"type": null|domain|regex|constraint|outlier, ...}
+        """detectors: list of dicts {"type": null|domain|regex|constraint|outlier|lof|sklearn, ...}
         given_cells: optional (positions, attrs) supplied by setErrorCells.
 
         Pass structure (the same on one GPU and on G shards; exchange() is the only cross-GPU step):
           local 1   fused NULL scan + histograms, constant / LUT detectors, per-key tables and projection
                     bits of the constraints, pair presence on a row sample
           exchange  [histograms | key tables | projection bits | presence bits]
-          local 2   constraint flags, detectors that need global counts; cell counts
+          local 2   constraint flags, detectors that need global counts (autofill domains, LOF); cell counts
           exchange  [cell counts]                                   (a few int64)
           local 3   exact tables of the undecided / selected pairs
           exchange  [pair tables]
@@ -900,6 +1010,10 @@ class Engine:
                     self.detect_constraints(det.get("path", ""), det.get("constraints", ""), tg, bitmaps, ex1, after)
                 elif kind == "outlier":
                     self.detect_outliers(tg, bitmaps, det.get("approx", False))
+                elif kind == "lof":
+                    self.detect_lof(tg, bitmaps, ex1, after)
+                elif kind == "sklearn":
+                    self.detect_sklearn(tg, bitmaps, det["factory"])
                 else:
                     raise ValueError("unknown detector type: {}".format(kind))
         # local 1 (cont.): one fused pass for the NULL bits of the discretised targets + every histogram,

@@ -6,7 +6,7 @@ A detector is a small value object; ``spec()`` lowers it to the dict the device 
 input registered in the catalog returns a pandas frame ``(row_id, attribute)``.
 """
 from abc import ABCMeta, abstractmethod
-from typing import Any, Dict, List, Optional
+from typing import Any, Callable, Dict, List, Optional
 
 from .utils import get_option_value
 
@@ -116,6 +116,59 @@ class GaussianOutlierErrorDetector(ErrorDetector):
 
     def spec(self):
         return {"type": "outlier", "approx": self.approx_enabled}
+
+
+class ScikitLearnBasedErrorDetector(ErrorDetector):
+    """Outlier detectors fitted on one continuous column at a time (errors.py:193-279): NULL cells are
+    filled with the column's median, and the cells labelled -1 are error cells.
+
+    ``parallel_mode_threshold`` / ``num_parallelism`` are validated and kept for compatibility but have no
+    effect: the reference fits per unseeded random partition above the threshold, here the fit is always
+    over the whole column (with ``num_parallelism=1`` the reference does the same)."""
+
+    def __init__(self, parallel_mode_threshold: int = 10000, num_parallelism: Optional[int] = None) -> None:
+        ErrorDetector.__init__(self)
+        if num_parallelism is not None and int(num_parallelism) <= 0:
+            raise ValueError("`num_parallelism` must be positive, got {}".format(num_parallelism))
+        self.parallel_mode_threshold = parallel_mode_threshold
+        self.num_parallelism = num_parallelism
+
+    def __str__(self) -> str:
+        return "{}()".format(self.__class__.__name__)
+
+
+class ScikitLearnBackedErrorDetector(ScikitLearnBasedErrorDetector):
+    """Any estimator with a scikit-learn-like ``fit_predict(X)`` returning 1 (inlier) / -1 (outlier),
+    built by ``error_detector_cls()`` once per column.  The user's object runs on the host over a host
+    copy of the column: this is the only detector that computes on the CPU, and it does not support
+    ``setDistributed`` runs."""
+
+    def __init__(self, error_detector_cls: Callable[[], Any], parallel_mode_threshold: int = 10000,
+                 num_parallelism: Optional[int] = None) -> None:
+        ScikitLearnBasedErrorDetector.__init__(self, parallel_mode_threshold, num_parallelism)
+        if not hasattr(error_detector_cls, "__call__"):
+            raise ValueError("`error_detector_cls` should be callable")
+        if not hasattr(error_detector_cls(), "fit_predict"):
+            raise ValueError("An instance that `error_detector_cls` returns should have a `fit_predict` method")
+        self.error_detector_cls = error_detector_cls
+
+    def spec(self):
+        return {"type": "sklearn", "factory": self.error_detector_cls}
+
+
+class LOFOutlierErrorDetector(ScikitLearnBasedErrorDetector):
+    """``sklearn.neighbors.LocalOutlierFactor(novelty=False)`` with its defaults (20 neighbours, euclidean
+    distance, contamination "auto") on each continuous target, computed exactly on the GPU over the
+    column's sorted distinct values (``dr_lof_score``).  Equal-distance ties at the edge of a neighbourhood
+    take the smaller value first (scikit-learn's choice follows its KD-tree traversal); a column with no
+    non-NULL value, or a table with fewer than two rows, yields no cells; a column holding +-inf raises
+    ``ValueError``."""
+
+    def __init__(self, parallel_mode_threshold: int = 10000, num_parallelism: Optional[int] = None) -> None:
+        ScikitLearnBasedErrorDetector.__init__(self, parallel_mode_threshold, num_parallelism)
+
+    def spec(self):
+        return {"type": "lof"}
 
 
 class ErrorModelOptions:
