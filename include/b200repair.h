@@ -516,6 +516,39 @@ int dr_tile_lut_fill(dr_ctx* ctx, int32_t* tile, int n_cols, int x_col, int y_co
 int dr_tile_fill_i32(dr_ctx* ctx, int32_t* tile, int n_cols, int col, const int32_t* cells, int64_t n_cells,
                      int32_t value, void* stream);
 
+/* ---- delphi.misc table utilities (RepairMiscApi.scala) ------------------------------------------
+ * dr_kmeans_assign: one k-means assignment over dictionary codes (splitInputTableInto :75-153).  P is
+ *   device float64 [p_rows][n_centres]: rows p_off[c] .. p_off[c] + dom[c] hold P_c = B_c mu^T for
+ *   column c (B_c: the q-gram counts of each dictionary entry, slot 0 = NULL -> all zeros).  A row's
+ *   score for centre j is mu_sq[j] - 2 * dot, dot = sum over c in table order (from 0.0, each add
+ *   rounded) of P[p_off[c] + code_c + 1][j]; ties go to the lower j.  split == NULL: every row takes the
+ *   best of all centres.  Otherwise (bisecting k-means) a row labelled L in [0, n_labels) with
+ *   split[L] = s >= 0 takes the better of s and s + 1, and every other row keeps its label.
+ *   labels: device int32 [n_rows], written in place.
+ * dr_label_counts: the centre-update counts of one column in global memory, for columns whose (label, value)
+ *   table does not fit dr_cooc's shared-memory tables: out[(label - lab_lo) * (dom + 1) + min(code + 1, dom)] += 1
+ *   for every row whose label lies in [lab_lo, lab_hi).  out: device int64 [lab_hi - lab_lo][dom + 1], zeroed
+ *   by the caller.
+ * dr_error_map: out (device uint8 [n_rows][n_attrs], row-major) = '*' where bit r of bitmaps[a] is set,
+ *   '-' elsewhere; bitmaps[a] == NULL means attribute a has no error (toErrorMap :316-347).
+ * dr_null_bits: IF(rand() > ratio, x, NULL) of injectNullAt (:155-182) on a validity bitmap that starts
+ *   at bit `bit_offset` (an Arrow array's offset).  Bit bit_offset + r of out = (valid == NULL or that bit
+ *   of valid) and u * 2^-53 > ratio, with u = splitmix64(row_base + r, key) >> 11; every other bit of
+ *   out's ceil((bit_offset + n_rows) / 32) words is 0.
+ * dr_flatten: flattenTable (:41-49): output row r * n_cols + c gets code_c(r) + base[c] (0 for NULL),
+ *   its validity bit, and row_ids[r] (r itself when row_ids is NULL). */
+int dr_kmeans_assign(dr_ctx* ctx, const int32_t* const* cols, const int32_t* dom, const int64_t* p_off, int n_cols,
+                     int64_t n_rows, const double* P, int64_t p_rows, const double* mu_sq, int32_t n_centres,
+                     const int32_t* split, int32_t n_labels, int32_t* labels, void* stream);
+int dr_label_counts(dr_ctx* ctx, const int32_t* labels, const int32_t* col, int32_t dom, int64_t n_rows,
+                    int32_t lab_lo, int32_t lab_hi, int64_t* out, void* stream);
+int dr_error_map(dr_ctx* ctx, const uint32_t* const* bitmaps, int n_attrs, int64_t n_rows, uint8_t* out,
+                 void* stream);
+int dr_null_bits(dr_ctx* ctx, const uint32_t* valid, int64_t bit_offset, int64_t n_rows, int64_t row_base,
+                 uint64_t key, double ratio, uint32_t* out, void* stream);
+int dr_flatten(dr_ctx* ctx, const int32_t* const* cols, const int64_t* base, int n_cols, int64_t n_rows,
+               const int64_t* row_ids, int32_t* out_codes, uint32_t* out_valid, int64_t* out_ids, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -5,7 +5,7 @@ shared library is missing, or no CUDA device is usable, every engine entry point
 """
 import ctypes
 import os
-from ctypes import POINTER, byref, c_char_p, c_double, c_int, c_int32, c_int64, c_void_p
+from ctypes import POINTER, byref, c_char_p, c_double, c_int, c_int32, c_int64, c_uint64, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_NAME = "libb200repair.so"
@@ -145,6 +145,13 @@ _SIGNATURES = {
                                 c_void_p, c_void_p]),
     "dr_tile_lut_fill": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_int32,
                                  c_void_p]),
+    "dr_kmeans_assign": (c_int, [c_void_p, _PP, POINTER(c_int32), POINTER(c_int64), c_int, c_int64, c_void_p, c_int64,
+                                 c_void_p, c_int32, c_void_p, c_int32, c_void_p, c_void_p]),
+    "dr_label_counts": (c_int, [c_void_p, c_void_p, c_void_p, c_int32, c_int64, c_int32, c_int32, c_void_p, c_void_p]),
+    "dr_error_map": (c_int, [c_void_p, _PP, c_int, c_int64, c_void_p, c_void_p]),
+    "dr_null_bits": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_uint64, c_double, c_void_p, c_void_p]),
+    "dr_flatten": (c_int, [c_void_p, _PP, POINTER(c_int64), c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
+                           c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(sorted(_SIGNATURES))
@@ -539,6 +546,33 @@ class Context:
         self._check(self.lib.dr_tile_lut_fill(self._h, _dp(tile), n_cols, x_col, y_col, _dp(cells), n_cells,
                                               _dp(lut), lut_size, self._stream()))
 
+    # ---- delphi.misc ------------------------------------------------------------------------------
+    def kmeans_assign(self, cols, dom, p_off, n_rows, P, mu_sq, labels, split=None):
+        """One k-means assignment over dictionary codes: P device float64 [p_rows][n_centres], mu_sq device
+        float64 [n_centres]; labels device int32, written in place (only rows split[label] >= 0 with split)."""
+        cp, _k = _ptr_array([c.data_ptr() for c in cols])
+        self._check(self.lib.dr_kmeans_assign(
+            self._h, cp, _i32_array(dom), _i64_array(p_off), len(cols), n_rows, _dp(P), int(P.shape[0]), _dp(mu_sq),
+            int(P.shape[1]), _dp(split), 0 if split is None else int(split.numel()), _dp(labels), self._stream()))
+
+    def label_counts(self, labels, col, dom, n_rows, lab_lo, lab_hi, out):
+        """out (device int64 [lab_hi - lab_lo][dom + 1], zeroed) += counts of (label, code slot)."""
+        self._check(self.lib.dr_label_counts(self._h, _dp(labels), _dp(col), dom, n_rows, lab_lo, lab_hi, _dp(out),
+                                             self._stream()))
+
+    def error_map(self, bitmaps, n_rows, out):
+        bp, _k = _ptr_array([0 if b is None else b.data_ptr() for b in bitmaps])
+        self._check(self.lib.dr_error_map(self._h, bp, len(bitmaps), n_rows, _dp(out), self._stream()))
+
+    def null_bits(self, valid, bit_offset, n_rows, row_base, key, ratio, out):
+        self._check(self.lib.dr_null_bits(self._h, _dp(valid), bit_offset, n_rows, row_base, key & ((1 << 64) - 1),
+                                          float(ratio), _dp(out), self._stream()))
+
+    def flatten(self, cols, base, n_rows, row_ids, out_codes, out_valid, out_ids):
+        cp, _k = _ptr_array([c.data_ptr() for c in cols])
+        self._check(self.lib.dr_flatten(self._h, cp, _i64_array(base), len(cols), n_rows, _dp(row_ids),
+                                        _dp(out_codes), _dp(out_valid), _dp(out_ids), self._stream()))
+
 
 def _profiled(name, fn):
     def wrapper(self, *args, **kwargs):
@@ -561,7 +595,8 @@ for _name in ("widen_u8", "h2d_copy", "d2h_copy", "index_presence", "index_remap
               "bitmap_andnot", "bitmap_count", "bitmap_count_many", "bitmap_to_rows_async", "bitmaps_to_rows_many", "bitmap_to_rows", "bitmap_rows_after_count", "tile_null_bitmaps", "changed_bitmap", "bitmap_gather", "bitmap_clear_rows", "discretize",
               "pair_presence", "cooc", "cooc_skip", "key_presence", "key_flag", "dc_exists", "combine_counts", "dc_lt_flag",
               "dc_hash_build", "dc_hash_flag", "domain_score", "domain_prune", "gather_rows_masked", "tile_null_bitmap", "gather",
-              "tile_gather", "lookup_sorted", "forest_predict", "forest_predict_ranked", "tile_fill", "gbdt_train"):
+              "tile_gather", "lookup_sorted", "forest_predict", "forest_predict_ranked", "tile_fill", "gbdt_train",
+              "kmeans_assign", "label_counts", "error_map", "null_bits", "flatten"):
     setattr(Context, _name, _profiled(_name, getattr(Context, _name)))
 
 

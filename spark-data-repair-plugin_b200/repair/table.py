@@ -177,6 +177,64 @@ def _sorted_dictionary(entries, used):
     return np.array(uniq, dtype=object), lut
 
 
+STRING_DEFAULT_SIZE = 20   # Spark's StringType.defaultSize
+
+
+def encode_columns(tbl):
+    """Every column of a ``pandas.DataFrame`` or ``pyarrow.Table`` label-encoded in schema order, with none of
+    checkInputTable's gates: the delphi.misc utilities take any table (RepairBase.scala:101-110).  Integer and
+    floating columns are numeric; everything else is encoded by its ``CAST(.. AS STRING)`` text.  Each Column
+    also carries ``default_size``: Spark's defaultSize of the source type (tinyint 1, smallint 2, int 4,
+    bigint 8, float 4, double 8; strings 20), which ``describe`` reports for numeric columns."""
+    import pandas as pd
+    cols = []
+    if isinstance(tbl, pd.DataFrame):
+        for c in tbl.columns:
+            s = tbl[c]
+            k = s.dtype.kind
+            kind = "int" if k in "iu" else "float" if k == "f" else None
+            size = int(getattr(s.dtype, "itemsize", 8)) if kind else 8
+            if kind is None and s.dtype == object:
+                # object columns holding only numbers (e.g. nullable ints collected from Spark) are numeric
+                non_null = [v for v in s.tolist() if v is not None and not (isinstance(v, float) and v != v)]
+                if non_null and all(isinstance(v, (int, np.integer)) and not isinstance(v, bool) for v in non_null):
+                    kind = "int"
+                elif non_null and all(isinstance(v, (int, float, np.integer, np.floating)) and
+                                      not isinstance(v, bool) for v in non_null):
+                    kind = "float"
+            if kind is not None:
+                arr = pd.to_numeric(s, errors="coerce").to_numpy(dtype=np.float64, na_value=np.nan)
+                col = _encode_numeric(str(c), kind, arr)
+            else:
+                if k == "b":
+                    s = s.map(lambda v: None if v is None or v != v else ("true" if v else "false"))
+                col = _encode_strings(str(c), s)
+                size = STRING_DEFAULT_SIZE
+            col.default_size = size
+            cols.append(col)
+        return cols
+    import pyarrow as pa
+    import pyarrow.compute as pc
+    for f in tbl.schema:
+        arr = tbl[f.name]
+        arr = arr.unify_dictionaries() if pa.types.is_dictionary(f.type) else arr
+        arr = arr.combine_chunks() if arr.num_chunks != 1 else arr.chunk(0)
+        t = f.type.value_type if pa.types.is_dictionary(f.type) else f.type
+        if pa.types.is_integer(t) or pa.types.is_floating(t):
+            if pa.types.is_dictionary(arr.type):
+                arr = arr.dictionary_decode()
+            vals = np.asarray(pc.cast(arr, pa.float64()).to_numpy(zero_copy_only=False), dtype=np.float64)
+            col = _encode_numeric(f.name, "int" if pa.types.is_integer(t) else "float", vals)
+            col.default_size = t.bit_width // 8
+        else:
+            if not (pa.types.is_string(t) or pa.types.is_large_string(t)):
+                arr = pc.cast(arr.dictionary_decode() if pa.types.is_dictionary(arr.type) else arr, pa.string())
+            col = _encode_arrow_strings(f.name, arr)
+            col.default_size = STRING_DEFAULT_SIZE
+        cols.append(col)
+    return cols
+
+
 class EncodedTable:
     """The collected input: row ids + encoded columns (row id excluded)."""
 
