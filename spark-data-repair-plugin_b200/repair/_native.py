@@ -2,8 +2,14 @@
 
 This is the only door into the hand-written sm_90a kernels.  There is no CPU fallback: if the
 shared library is missing, or no CUDA device is usable, every engine entry point raises.
+
+Adding an entry point: declare it in the header, give it a row in ``_SIGNATURES`` (the argument
+kinds below do the marshalling), and add a ``Context`` method -- one ``_call`` when the Python
+arguments map one-to-one onto the C ones.  Every public ``Context`` method outside ``_NOT_PROFILED`` is
+profiled.
 """
 import ctypes
+import functools
 import os
 from ctypes import POINTER, byref, c_char_p, c_double, c_int, c_int32, c_int64, c_uint64, c_void_p
 
@@ -54,7 +60,47 @@ class dr_gbdt_params(ctypes.Structure):
                 ("subsample_freq", c_int32), ("seed", c_int32)]
 
 
-_PP = POINTER(c_void_p)
+# ---- argument kinds --------------------------------------------------------------------------------
+# Pointer-width ctypes types whose from_param converts a Python value at call time.  ctypes keeps what
+# from_param returns alive until the C function returns, so the host arrays built here need no other
+# reference.
+def _address(buf):
+    return buf if buf is None or isinstance(buf, int) else buf.data_ptr()
+
+
+class _Buf(c_void_p):
+    """A buffer: a torch tensor (its data_ptr()), an integer address, or None for NULL."""
+
+    @classmethod
+    def from_param(cls, buf):
+        return c_void_p(_address(buf))
+
+
+class _Bufs(c_void_p):
+    """A list of buffers, each as _Buf takes it, passed as a host void* array."""
+
+    @classmethod
+    def from_param(cls, bufs):
+        return (c_void_p * max(len(bufs), 1))(*[_address(b) for b in bufs])
+
+
+class _Ints(c_void_p):
+    """A list of integers passed as a host array of _elem, or None for NULL."""
+    _elem = None
+
+    @classmethod
+    def from_param(cls, vals):
+        return None if vals is None else (cls._elem * max(len(vals), 1))(*[int(v) for v in vals])
+
+
+class _I32s(_Ints):
+    _elem = c_int32
+
+
+class _I64s(_Ints):
+    _elem = c_int64
+
+
 _SIGNATURES = {
     # name: (restype, argtypes)
     "dr_ctx_create": (c_int, [c_int, POINTER(c_void_p)]),
@@ -62,96 +108,84 @@ _SIGNATURES = {
     "dr_last_error": (c_char_p, [c_void_p]),
     "dr_abi_version": (c_int, []),
     "dr_launch_count": (c_int64, [c_void_p]),
-    "dr_widen_u8": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
-    "dr_h2d_copy": (c_int, [c_void_p, _PP, _PP, POINTER(c_int64), c_int, c_int, c_void_p]),
-    "dr_d2h_copy": (c_int, [c_void_p, _PP, _PP, POINTER(c_int64), c_int, c_int, c_void_p]),
-    "dr_index_presence": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int64, c_int64, c_int32, c_void_p, c_void_p]),
-    "dr_index_remap": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int64, c_int64, c_void_p, c_int32,
-                               c_void_p, c_void_p]),
-    "dr_ids_unique_i64": (c_int, [c_void_p, c_void_p, c_int64, POINTER(c_int), c_void_p]),
-    "dr_gather_i64": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
-    "dr_valid_bits": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
-    "dr_scan_hist": (c_int, [c_void_p, _PP, POINTER(c_int32), c_int, c_int64, _PP, c_void_p, c_void_p]),
-    "dr_lut_scan": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int32, c_void_p, c_void_p]),
-    "dr_quartiles": (c_int, [c_void_p, c_void_p, c_int64, POINTER(c_double), POINTER(c_int64), c_void_p]),
-    "dr_range_flag": (c_int, [c_void_p, c_void_p, c_int64, c_double, c_double, c_void_p, c_void_p]),
-    "dr_lof_score": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
-                             c_void_p]),
-    "dr_lof_median": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, POINTER(c_int64), c_void_p]),
-    "dr_lof_flag": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int32, c_int32, c_void_p, c_void_p]),
-    "dr_dc_const": (c_int, [c_void_p, _PP, POINTER(c_int32), POINTER(c_int32), c_int, c_int64, c_void_p, c_void_p]),
-    "dr_dc_fd_build": (c_int, [c_void_p, _PP, POINTER(c_int64), c_int, c_void_p, c_int64, c_int64, c_void_p,
-                               c_void_p, c_void_p]),
-    "dr_dc_fd_flag": (c_int, [c_void_p, _PP, POINTER(c_int64), c_int, c_int64, c_int64, c_void_p, c_void_p,
-                              c_void_p, c_void_p]),
-    "dr_dc_hash_build": (c_int, [c_void_p, _PP, POINTER(c_int64), c_int, c_void_p, c_int64, c_int64, c_void_p,
-                                 c_void_p, c_void_p, c_void_p]),
-    "dr_dc_hash_flag": (c_int, [c_void_p, _PP, POINTER(c_int64), c_int, c_void_p, c_int, c_int64, c_int64, c_void_p,
-                                c_void_p, c_void_p, c_void_p, c_void_p]),
-    "dr_dc_lt_flag": (c_int, [c_void_p, _PP, POINTER(c_int64), c_int, c_void_p, c_int64, c_int64, c_void_p,
-                              c_void_p, c_void_p]),
-    "dr_bitmap_or": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
-    "dr_bitmap_andnot": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
-    "dr_bitmap_count": (c_int, [c_void_p, c_void_p, c_int64, POINTER(c_int64), c_void_p]),
-    "dr_bitmap_count_many": (c_int, [c_void_p, _PP, c_int, c_int64, POINTER(c_int64), c_void_p]),
-    "dr_bitmap_to_rows_async": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_void_p]),
-    "dr_bitmaps_to_rows_many": (c_int, [c_void_p, _PP, c_int, c_int64, _PP, POINTER(c_int64), c_void_p]),
-    "dr_bitmap_to_rows": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int64, POINTER(c_int64), c_void_p]),
-    "dr_bitmap_rows_after_count": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_void_p]),
-    "dr_tile_null_bitmaps": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int64, c_void_p, c_void_p]),
-    "dr_changed_bitmap": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
-    "dr_bitmap_gather": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
-    "dr_bitmap_clear_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
-    "dr_discretize": (c_int, [c_void_p, c_void_p, c_int64, c_double, c_double, c_int32, c_void_p, c_void_p]),
-    "dr_pair_presence": (c_int, [c_void_p, _PP, POINTER(c_int32), c_int, POINTER(c_int32), POINTER(c_int32), c_int,
-                                 POINTER(c_int64), c_int64, c_int64, c_int64, c_void_p, c_void_p]),
-    "dr_cooc": (c_int, [c_void_p, _PP, POINTER(c_int32), c_int, POINTER(c_int32), POINTER(c_int32), c_int,
-                        POINTER(c_int64), c_int64, c_void_p, c_void_p]),
-    "dr_domain_score": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int32, _PP, POINTER(c_int32), _PP, c_int,
-                                c_void_p, POINTER(c_int64), c_int64, c_double, c_void_p, c_void_p, c_void_p,
-                                c_void_p]),
-    "dr_domain_prune": (c_int, [c_void_p, POINTER(dr_domain_target), c_int, c_int64, c_int64, c_double, c_void_p,
-                                c_void_p]),
-    "dr_gather_rows_masked": (c_int, [c_void_p, _PP, _PP, c_int, c_void_p, c_int64, c_void_p, c_void_p]),
-    "dr_gather_rows_masked_f64": (c_int, [c_void_p, _PP, _PP, c_int, c_void_p, c_int64, c_void_p, c_void_p]),
-    "dr_gather_rows_masked_nulls": (c_int, [c_void_p, _PP, _PP, c_int, c_void_p, c_int64, c_void_p, c_void_p,
-                                            c_int64, c_void_p]),
-    "dr_tile_null_bitmap": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p]),
-    "dr_tile_null_bitmap_f64": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p]),
-    "dr_gather_i32": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
-    "dr_gather_f64": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
-    "dr_tile_gather_i32": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p]),
-    "dr_tile_gather_f64": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p]),
-    "dr_lookup_sorted": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p]),
-    "dr_forest_predict": (c_int, [c_void_p, POINTER(dr_forest), c_void_p, c_int, c_void_p, c_int, c_void_p, c_int64,
-                                  c_int, c_void_p, c_void_p]),
-    "dr_cooc_skip": (c_int, [c_void_p, _PP, POINTER(c_int32), c_int, POINTER(c_int32), POINTER(c_int32), c_int,
-                             POINTER(c_int64), c_int64, c_void_p, POINTER(c_int64), c_void_p, c_void_p]),
-    "dr_key_presence": (c_int, [c_void_p, _PP, POINTER(c_int64), c_int, c_int64, c_int64, c_void_p, c_void_p]),
-    "dr_key_flag": (c_int, [c_void_p, _PP, POINTER(c_int64), c_int, c_int64, c_int64, c_void_p, c_void_p, c_void_p]),
-    "dr_dc_exists": (c_int, [c_void_p, _PP, _PP, POINTER(c_int32), c_int, c_int64, c_void_p, c_void_p, c_void_p,
-                             c_void_p]),
-    "dr_combine_counts": (c_int, [c_void_p, c_void_p, c_int, c_int64, POINTER(c_int64), POINTER(c_int32), c_int,
-                                  c_void_p, c_void_p]),
-    "dr_forest_predict_ranked": (c_int, [c_void_p, POINTER(dr_forest_ranked), c_void_p, c_int, c_void_p, c_int64,
-                                         c_int, c_void_p, c_void_p]),
-    "dr_gbdt_workspace_bytes": (c_int64, [c_int32, c_int32]),
-    "dr_gbdt_train": (c_int, [c_void_p, POINTER(dr_gbdt_params), c_void_p, POINTER(c_int32), c_void_p, c_void_p,
-                              c_void_p, POINTER(c_double), c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
-    "dr_tile_fill_i32": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_int64, c_int32, c_void_p]),
-    "dr_scatter_i32": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
-    "dr_scatter_f64": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
-    "dr_fd_map_build": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_void_p,
-                                c_void_p, c_void_p]),
-    "dr_tile_lut_fill": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_int32,
+    "dr_widen_u8": (c_int, [c_void_p, _Buf, c_int64, _Buf, c_void_p]),
+    "dr_h2d_copy": (c_int, [c_void_p, _Bufs, _Bufs, _I64s, c_int, c_int, c_void_p]),
+    "dr_d2h_copy": (c_int, [c_void_p, _Bufs, _Bufs, _I64s, c_int, c_int, c_void_p]),
+    "dr_index_presence": (c_int, [c_void_p, _Buf, c_int, _Buf, c_int64, c_int64, c_int32, _Buf, c_void_p]),
+    "dr_index_remap": (c_int, [c_void_p, _Buf, c_int, _Buf, c_int64, c_int64, _Buf, c_int32, _Buf, c_void_p]),
+    "dr_ids_unique_i64": (c_int, [c_void_p, _Buf, c_int64, POINTER(c_int), c_void_p]),
+    "dr_gather_i64": (c_int, [c_void_p, _Buf, _Buf, c_int64, _Buf, c_void_p]),
+    "dr_valid_bits": (c_int, [c_void_p, _Buf, c_int64, _Buf, c_void_p]),
+    "dr_scan_hist": (c_int, [c_void_p, _Bufs, _I32s, c_int, c_int64, _Bufs, _Buf, c_void_p]),
+    "dr_lut_scan": (c_int, [c_void_p, _Buf, c_int64, _Buf, c_int32, _Buf, c_void_p]),
+    "dr_quartiles": (c_int, [c_void_p, _Buf, c_int64, POINTER(c_double), POINTER(c_int64), c_void_p]),
+    "dr_range_flag": (c_int, [c_void_p, _Buf, c_int64, c_double, c_double, _Buf, c_void_p]),
+    "dr_lof_score": (c_int, [c_void_p, _Buf, _Buf, c_int64, c_int32, _Buf, _Buf, _Buf, _Buf, c_void_p]),
+    "dr_lof_median": (c_int, [c_void_p, _Buf, c_int64, c_int64, c_int64, POINTER(c_int64), c_void_p]),
+    "dr_lof_flag": (c_int, [c_void_p, _Buf, c_int64, _Buf, c_int32, c_int32, _Buf, c_void_p]),
+    "dr_dc_const": (c_int, [c_void_p, _Bufs, _I32s, _I32s, c_int, c_int64, _Buf, c_void_p]),
+    "dr_dc_fd_build": (c_int, [c_void_p, _Bufs, _I64s, c_int, _Buf, c_int64, c_int64, _Buf, _Buf, c_void_p]),
+    "dr_dc_fd_flag": (c_int, [c_void_p, _Bufs, _I64s, c_int, c_int64, c_int64, _Buf, _Buf, _Buf, c_void_p]),
+    "dr_dc_hash_build": (c_int, [c_void_p, _Bufs, _I64s, c_int, _Buf, c_int64, c_int64, _Buf, _Buf, _Buf,
                                  c_void_p]),
-    "dr_kmeans_assign": (c_int, [c_void_p, _PP, POINTER(c_int32), POINTER(c_int64), c_int, c_int64, c_void_p, c_int64,
-                                 c_void_p, c_int32, c_void_p, c_int32, c_void_p, c_void_p]),
-    "dr_label_counts": (c_int, [c_void_p, c_void_p, c_void_p, c_int32, c_int64, c_int32, c_int32, c_void_p, c_void_p]),
-    "dr_error_map": (c_int, [c_void_p, _PP, c_int, c_int64, c_void_p, c_void_p]),
-    "dr_null_bits": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_uint64, c_double, c_void_p, c_void_p]),
-    "dr_flatten": (c_int, [c_void_p, _PP, POINTER(c_int64), c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
-                           c_void_p]),
+    "dr_dc_hash_flag": (c_int, [c_void_p, _Bufs, _I64s, c_int, _Buf, c_int, c_int64, c_int64, _Buf, _Buf, _Buf,
+                                _Buf, c_void_p]),
+    "dr_dc_lt_flag": (c_int, [c_void_p, _Bufs, _I64s, c_int, _Buf, c_int64, c_int64, _Buf, _Buf, c_void_p]),
+    "dr_bitmap_or": (c_int, [c_void_p, _Buf, _Buf, c_int64, c_void_p]),
+    "dr_bitmap_andnot": (c_int, [c_void_p, _Buf, _Buf, c_int64, c_void_p]),
+    "dr_bitmap_count": (c_int, [c_void_p, _Buf, c_int64, POINTER(c_int64), c_void_p]),
+    "dr_bitmap_count_many": (c_int, [c_void_p, _Bufs, c_int, c_int64, POINTER(c_int64), c_void_p]),
+    "dr_bitmap_to_rows_async": (c_int, [c_void_p, _Buf, c_int64, _Buf, c_int64, c_void_p]),
+    "dr_bitmaps_to_rows_many": (c_int, [c_void_p, _Bufs, c_int, c_int64, _Bufs, _I64s, c_void_p]),
+    "dr_bitmap_to_rows": (c_int, [c_void_p, _Buf, c_int64, _Buf, c_int64, POINTER(c_int64), c_void_p]),
+    "dr_bitmap_rows_after_count": (c_int, [c_void_p, _Buf, c_int64, _Buf, c_int64, c_void_p]),
+    "dr_tile_null_bitmaps": (c_int, [c_void_p, _Buf, c_int64, c_int, c_int64, _Buf, c_void_p]),
+    "dr_changed_bitmap": (c_int, [c_void_p, _Buf, _Buf, c_int64, _Buf, c_void_p]),
+    "dr_bitmap_gather": (c_int, [c_void_p, _Buf, _Buf, c_int64, _Buf, c_void_p]),
+    "dr_bitmap_clear_rows": (c_int, [c_void_p, _Buf, _Buf, _Buf, c_int64, c_void_p]),
+    "dr_discretize": (c_int, [c_void_p, _Buf, c_int64, c_double, c_double, c_int32, _Buf, c_void_p]),
+    "dr_pair_presence": (c_int, [c_void_p, _Bufs, _I32s, c_int, _I32s, _I32s, c_int, _I64s, c_int64, c_int64,
+                                 c_int64, _Buf, c_void_p]),
+    "dr_cooc": (c_int, [c_void_p, _Bufs, _I32s, c_int, _I32s, _I32s, c_int, _I64s, c_int64, _Buf, c_void_p]),
+    "dr_domain_score": (c_int, [c_void_p, _Buf, c_int64, _Buf, c_int32, _Bufs, _I32s, _Bufs, c_int, _Buf, _I64s,
+                                c_int64, c_double, _Buf, _Buf, _Buf, c_void_p]),
+    "dr_domain_prune": (c_int, [c_void_p, POINTER(dr_domain_target), c_int, c_int64, c_int64, c_double, _Buf,
+                                c_void_p]),
+    "dr_gather_rows_masked": (c_int, [c_void_p, _Bufs, _Bufs, c_int, _Buf, c_int64, _Buf, c_void_p]),
+    "dr_gather_rows_masked_f64": (c_int, [c_void_p, _Bufs, _Bufs, c_int, _Buf, c_int64, _Buf, c_void_p]),
+    "dr_gather_rows_masked_nulls": (c_int, [c_void_p, _Bufs, _Bufs, c_int, _Buf, c_int64, _Buf, _Buf, c_int64,
+                                            c_void_p]),
+    "dr_tile_null_bitmap": (c_int, [c_void_p, _Buf, c_int64, c_int, c_int, _Buf, c_void_p]),
+    "dr_tile_null_bitmap_f64": (c_int, [c_void_p, _Buf, c_int64, c_int, c_int, _Buf, c_void_p]),
+    "dr_gather_i32": (c_int, [c_void_p, _Buf, _Buf, c_int64, _Buf, c_void_p]),
+    "dr_gather_f64": (c_int, [c_void_p, _Buf, _Buf, c_int64, _Buf, c_void_p]),
+    "dr_tile_gather_i32": (c_int, [c_void_p, _Buf, c_int, c_int, _Buf, c_int64, _Buf, c_void_p]),
+    "dr_tile_gather_f64": (c_int, [c_void_p, _Buf, c_int, c_int, _Buf, c_int64, _Buf, c_void_p]),
+    "dr_lookup_sorted": (c_int, [c_void_p, _Buf, c_int64, _Buf, c_int64, _Buf, c_void_p]),
+    "dr_forest_predict": (c_int, [c_void_p, POINTER(dr_forest), _Buf, c_int, _Buf, c_int, _Buf, c_int64, c_int,
+                                  _Buf, c_void_p]),
+    "dr_cooc_skip": (c_int, [c_void_p, _Bufs, _I32s, c_int, _I32s, _I32s, c_int, _I64s, c_int64, _Buf, _I64s,
+                             _Buf, c_void_p]),
+    "dr_key_presence": (c_int, [c_void_p, _Bufs, _I64s, c_int, c_int64, c_int64, _Buf, c_void_p]),
+    "dr_key_flag": (c_int, [c_void_p, _Bufs, _I64s, c_int, c_int64, c_int64, _Buf, _Buf, c_void_p]),
+    "dr_dc_exists": (c_int, [c_void_p, _Bufs, _Bufs, _I32s, c_int, c_int64, _Buf, _Buf, _Buf, c_void_p]),
+    "dr_combine_counts": (c_int, [c_void_p, _Buf, c_int, c_int64, _I64s, _I32s, c_int, _Buf, c_void_p]),
+    "dr_forest_predict_ranked": (c_int, [c_void_p, POINTER(dr_forest_ranked), _Buf, c_int, _Buf, c_int64, c_int,
+                                         _Buf, c_void_p]),
+    "dr_gbdt_workspace_bytes": (c_int64, [c_int32, c_int32]),
+    "dr_gbdt_train": (c_int, [c_void_p, POINTER(dr_gbdt_params), _Buf, _I32s, _Buf, _Buf, _Buf, POINTER(c_double),
+                              _Buf, c_int64, _Buf, _Buf, c_void_p]),
+    "dr_tile_fill_i32": (c_int, [c_void_p, _Buf, c_int, c_int, _Buf, c_int64, c_int32, c_void_p]),
+    "dr_scatter_i32": (c_int, [c_void_p, _Buf, _Buf, _Buf, c_int64, c_void_p]),
+    "dr_scatter_f64": (c_int, [c_void_p, _Buf, _Buf, _Buf, c_int64, c_void_p]),
+    "dr_fd_map_build": (c_int, [c_void_p, _Buf, _Buf, _Buf, _Buf, c_int64, c_int32, _Buf, _Buf, c_void_p]),
+    "dr_tile_lut_fill": (c_int, [c_void_p, _Buf, c_int, c_int, c_int, _Buf, c_int64, _Buf, c_int32, c_void_p]),
+    "dr_kmeans_assign": (c_int, [c_void_p, _Bufs, _I32s, _I64s, c_int, c_int64, _Buf, c_int64, _Buf, c_int32, _Buf,
+                                 c_int32, _Buf, c_void_p]),
+    "dr_label_counts": (c_int, [c_void_p, _Buf, _Buf, c_int32, c_int64, c_int32, c_int32, _Buf, c_void_p]),
+    "dr_error_map": (c_int, [c_void_p, _Bufs, c_int, c_int64, _Buf, c_void_p]),
+    "dr_null_bits": (c_int, [c_void_p, _Buf, c_int64, c_int64, c_int64, c_uint64, c_double, _Buf, c_void_p]),
+    "dr_flatten": (c_int, [c_void_p, _Bufs, _I64s, c_int, c_int64, _Buf, _Buf, _Buf, _Buf, c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(sorted(_SIGNATURES))
@@ -175,26 +209,6 @@ def load_library():
         fn.argtypes = argtypes
     _lib = lib
     return lib
-
-
-def _ptr_array(ptrs):
-    arr = (c_void_p * max(len(ptrs), 1))()
-    for i, p in enumerate(ptrs):
-        arr[i] = p
-    return ctypes.cast(arr, _PP), arr
-
-
-def _i32_array(vals):
-    return (c_int32 * max(len(vals), 1))(*[int(v) for v in vals])
-
-
-def _i64_array(vals):
-    return (c_int64 * max(len(vals), 1))(*[int(v) for v in vals])
-
-
-def _dp(t):
-    """device pointer of a torch tensor (None -> NULL)."""
-    return None if t is None else c_void_p(t.data_ptr())
 
 
 class Context:
@@ -247,130 +261,103 @@ class Context:
         except Exception:
             pass
 
-    def _check(self, rc):
-        if rc != 0:
-            raise NativeError("libb200repair: " + self.lib.dr_last_error(self._h).decode())
-
-    @staticmethod
-    def _stream():
+    def _call(self, name, *args):
+        """lib.<name>(context, *args, current torch stream); raises NativeError on a non-zero return code."""
         import torch
-        return c_void_p(torch.cuda.current_stream().cuda_stream)
+        if getattr(self.lib, name)(self._h, *args, torch.cuda.current_stream().cuda_stream) != 0:
+            raise NativeError("libb200repair: " + self.lib.dr_last_error(self._h).decode())
 
     @property
     def launch_count(self):
         return int(self.lib.dr_launch_count(self._h))
 
     def widen_u8(self, src, n, dst):
-        self._check(self.lib.dr_widen_u8(self._h, _dp(src), n, _dp(dst), self._stream()))
+        self._call("dr_widen_u8", src, n, dst)
 
     # ---- Arrow ingest / egress ---------------------------------------------------------------------
     def h2d_copy(self, host_ptrs, dev_tensors_or_ptrs, nbytes, threads=0):
         """Pageable host buffers (addresses) -> device (tensors or addresses); blocks until complete."""
-        sp, _k1 = _ptr_array(host_ptrs)
-        dp, _k2 = _ptr_array([d if isinstance(d, int) else d.data_ptr() for d in dev_tensors_or_ptrs])
-        self._check(self.lib.dr_h2d_copy(self._h, sp, dp, _i64_array(nbytes), len(host_ptrs), threads, self._stream()))
+        self._call("dr_h2d_copy", host_ptrs, dev_tensors_or_ptrs, nbytes, len(host_ptrs), threads)
 
     def d2h_copy(self, dev_tensors_or_ptrs, host_ptrs, nbytes, threads=0):
-        sp, _k1 = _ptr_array([d if isinstance(d, int) else d.data_ptr() for d in dev_tensors_or_ptrs])
-        dp, _k2 = _ptr_array(host_ptrs)
-        self._check(self.lib.dr_d2h_copy(self._h, sp, dp, _i64_array(nbytes), len(host_ptrs), threads, self._stream()))
+        self._call("dr_d2h_copy", dev_tensors_or_ptrs, host_ptrs, nbytes, len(host_ptrs), threads)
 
     def index_presence(self, idx_ptr, width, validity_ptr, bit_offset, n_rows, dict_size, used):
-        self._check(self.lib.dr_index_presence(self._h, c_void_p(idx_ptr), width, c_void_p(validity_ptr or 0),
-                                               bit_offset, n_rows, dict_size, _dp(used), self._stream()))
+        self._call("dr_index_presence", idx_ptr, width, validity_ptr, bit_offset, n_rows, dict_size, used)
 
     def index_remap(self, idx_ptr, width, validity_ptr, bit_offset, n_rows, lut_ptr, dict_size, dst_ptr):
-        self._check(self.lib.dr_index_remap(self._h, c_void_p(idx_ptr), width, c_void_p(validity_ptr or 0), bit_offset,
-                                            n_rows, c_void_p(lut_ptr), dict_size, c_void_p(dst_ptr), self._stream()))
+        self._call("dr_index_remap", idx_ptr, width, validity_ptr, bit_offset, n_rows, lut_ptr, dict_size, dst_ptr)
 
     def ids_unique(self, ids, n):
         out = c_int()
-        self._check(self.lib.dr_ids_unique_i64(self._h, _dp(ids), n, byref(out), self._stream()))
+        self._call("dr_ids_unique_i64", ids, n, byref(out))
         return bool(out.value)
 
     def gather_i64(self, col, rows, n, out):
-        self._check(self.lib.dr_gather_i64(self._h, _dp(col), _dp(rows), n, _dp(out), self._stream()))
+        self._call("dr_gather_i64", col, rows, n, out)
 
     def valid_bits(self, codes, n, bits):
-        self._check(self.lib.dr_valid_bits(self._h, _dp(codes), n, _dp(bits), self._stream()))
+        self._call("dr_valid_bits", codes, n, bits)
 
     # ---- detectors -------------------------------------------------------------------------------
     def scan_hist(self, cols, dom, n_rows, bitmaps, hist):
-        cp, _k1 = _ptr_array([c.data_ptr() for c in cols])
-        bp, _k2 = _ptr_array([0 if b is None else b.data_ptr() for b in bitmaps])
-        self._check(self.lib.dr_scan_hist(self._h, cp, _i32_array(dom), len(cols), n_rows, bp, _dp(hist),
-                                          self._stream()))
+        self._call("dr_scan_hist", cols, dom, len(cols), n_rows, bitmaps, hist)
 
     def lut_scan(self, col, n_rows, lut, dict_size, bitmap):
-        self._check(self.lib.dr_lut_scan(self._h, _dp(col), n_rows, _dp(lut), dict_size, _dp(bitmap), self._stream()))
+        self._call("dr_lut_scan", col, n_rows, lut, dict_size, bitmap)
 
     def quartiles(self, col, n_rows):
         q = (c_double * 2)()
         n = c_int64()
-        self._check(self.lib.dr_quartiles(self._h, _dp(col), n_rows, q, byref(n), self._stream()))
+        self._call("dr_quartiles", col, n_rows, q, byref(n))
         return float(q[0]), float(q[1]), int(n.value)
 
     def range_flag(self, col, n_rows, lower, upper, bitmap):
-        self._check(self.lib.dr_range_flag(self._h, _dp(col), n_rows, lower, upper, _dp(bitmap), self._stream()))
+        self._call("dr_range_flag", col, n_rows, lower, upper, bitmap)
 
     def lof_score(self, u, cnt, k, verdict, kdist, lrd, lof=None):
         """LOF over sorted distinct values u (float64) with multiplicities cnt (int64), all device tensors of
         one length; writes verdict (uint8, 1 = outlier), kdist and lrd, and lof when given."""
-        self._check(self.lib.dr_lof_score(self._h, _dp(u), _dp(cnt), int(u.numel()), int(k), _dp(verdict),
-                                          _dp(kdist), _dp(lrd), _dp(lof), self._stream()))
+        self._call("dr_lof_score", u, cnt, int(u.numel()), int(k), verdict, kdist, lrd, lof)
 
     def lof_median(self, cnt, r0, r1):
         """-> (entry holding rank r0, entry holding rank r1) of the multiset counted by cnt (device int64)."""
         out = (c_int64 * 2)()
-        self._check(self.lib.dr_lof_median(self._h, _dp(cnt), int(cnt.numel()), int(r0), int(r1), out,
-                                           self._stream()))
+        self._call("dr_lof_median", cnt, int(cnt.numel()), int(r0), int(r1), out)
         return int(out[0]), int(out[1])
 
     def lof_flag(self, col, n_rows, verdict, dict_size, null_verdict, bitmap):
-        self._check(self.lib.dr_lof_flag(self._h, _dp(col), n_rows, _dp(verdict), dict_size, int(bool(null_verdict)),
-                                         _dp(bitmap), self._stream()))
+        self._call("dr_lof_flag", col, n_rows, verdict, dict_size, int(bool(null_verdict)), bitmap)
 
     def dc_const(self, cols, ops, args, n_rows, row_bitmap):
-        cp, _k = _ptr_array([c.data_ptr() for c in cols])
-        self._check(self.lib.dr_dc_const(self._h, cp, _i32_array(ops), _i32_array(args), len(cols), n_rows,
-                                         _dp(row_bitmap), self._stream()))
+        self._call("dr_dc_const", cols, ops, args, len(cols), n_rows, row_bitmap)
 
     def dc_fd_build(self, key_cols, strides, b_col, n_rows, key_space, lo, hi):
-        cp, _k = _ptr_array([c.data_ptr() for c in key_cols])
-        self._check(self.lib.dr_dc_fd_build(self._h, cp, _i64_array(strides), len(key_cols), _dp(b_col), n_rows,
-                                            key_space, _dp(lo), _dp(hi), self._stream()))
+        self._call("dr_dc_fd_build", key_cols, strides, len(key_cols), b_col, n_rows, key_space, lo, hi)
 
     def dc_fd_flag(self, key_cols, strides, n_rows, key_space, lo, hi, row_bitmap):
-        cp, _k = _ptr_array([c.data_ptr() for c in key_cols])
-        self._check(self.lib.dr_dc_fd_flag(self._h, cp, _i64_array(strides), len(key_cols), n_rows, key_space,
-                                           _dp(lo), _dp(hi), _dp(row_bitmap), self._stream()))
+        self._call("dr_dc_fd_flag", key_cols, strides, len(key_cols), n_rows, key_space, lo, hi, row_bitmap)
 
     def dc_hash_build(self, key_cols, strides, b_col, n_rows, capacity, table_keys, lo, hi):
-        cp, _k = _ptr_array([c.data_ptr() for c in key_cols])
-        self._check(self.lib.dr_dc_hash_build(self._h, cp, _i64_array(strides), len(key_cols), _dp(b_col), n_rows,
-                                              capacity, _dp(table_keys), _dp(lo), _dp(hi), self._stream()))
+        self._call("dr_dc_hash_build", key_cols, strides, len(key_cols), b_col, n_rows, capacity, table_keys, lo, hi)
 
     def dc_hash_flag(self, key_cols, strides, x_col, mode, n_rows, capacity, table_keys, lo, hi, row_bitmap):
-        cp, _k = _ptr_array([c.data_ptr() for c in key_cols])
-        self._check(self.lib.dr_dc_hash_flag(self._h, cp, _i64_array(strides), len(key_cols), _dp(x_col), mode, n_rows,
-                                             capacity, _dp(table_keys), _dp(lo), _dp(hi), _dp(row_bitmap),
-                                             self._stream()))
+        self._call("dr_dc_hash_flag", key_cols, strides, len(key_cols), x_col, mode, n_rows, capacity, table_keys,
+                   lo, hi, row_bitmap)
 
     def dc_lt_flag(self, key_cols, strides, x_col, n_rows, key_space, hi, row_bitmap):
-        cp, _k = _ptr_array([c.data_ptr() for c in key_cols])
-        self._check(self.lib.dr_dc_lt_flag(self._h, cp, _i64_array(strides), len(key_cols), _dp(x_col), n_rows,
-                                           key_space, _dp(hi), _dp(row_bitmap), self._stream()))
+        self._call("dr_dc_lt_flag", key_cols, strides, len(key_cols), x_col, n_rows, key_space, hi, row_bitmap)
 
     # ---- bitmaps ---------------------------------------------------------------------------------
     def bitmap_or(self, dst, src, n_rows):
-        self._check(self.lib.dr_bitmap_or(self._h, _dp(dst), _dp(src), n_rows, self._stream()))
+        self._call("dr_bitmap_or", dst, src, n_rows)
 
     def bitmap_andnot(self, dst, src, n_rows):
-        self._check(self.lib.dr_bitmap_andnot(self._h, _dp(dst), _dp(src), n_rows, self._stream()))
+        self._call("dr_bitmap_andnot", dst, src, n_rows)
 
     def bitmap_count(self, bitmap, n_rows):
         n = c_int64()
-        self._check(self.lib.dr_bitmap_count(self._h, _dp(bitmap), n_rows, byref(n), self._stream()))
+        self._call("dr_bitmap_count", bitmap, n_rows, byref(n))
         return int(n.value)
 
     def bitmap_count_many(self, bitmaps, n_rows):
@@ -378,203 +365,161 @@ class Context:
         out = []
         for i in range(0, len(bitmaps), 128):
             part = bitmaps[i:i + 128]
-            bp, _keep = _ptr_array([b.data_ptr() for b in part])
             counts = (c_int64 * len(part))()
-            self._check(self.lib.dr_bitmap_count_many(self._h, bp, len(part), n_rows, counts, self._stream()))
+            self._call("dr_bitmap_count_many", part, len(part), n_rows, counts)
             out += [int(c) for c in counts]
         return out
 
     def bitmap_to_rows_async(self, bitmap, n_rows, out_rows, count):
         """Ordered compaction of a bitmap whose popcount is known: no host synchronisation."""
-        self._check(self.lib.dr_bitmap_to_rows_async(self._h, _dp(bitmap), n_rows, _dp(out_rows), count,
-                                                     self._stream()))
+        self._call("dr_bitmap_to_rows_async", bitmap, n_rows, out_rows, count)
 
     def bitmaps_to_rows_many(self, bitmaps, n_rows, outs, counts):
         """Ordered compaction of several bitmaps with known popcounts (three launches per 128 bitmaps)."""
         for i in range(0, len(bitmaps), 128):
-            bp, _k1 = _ptr_array([b.data_ptr() for b in bitmaps[i:i + 128]])
-            op, _k2 = _ptr_array([o.data_ptr() if c else 0 for o, c in zip(outs[i:i + 128], counts[i:i + 128])])
-            self._check(self.lib.dr_bitmaps_to_rows_many(self._h, bp, len(bitmaps[i:i + 128]), n_rows, op,
-                                                         _i64_array(counts[i:i + 128]), self._stream()))
+            part, part_counts = bitmaps[i:i + 128], counts[i:i + 128]
+            part_outs = [o if c else None for o, c in zip(outs[i:i + 128], part_counts)]
+            self._call("dr_bitmaps_to_rows_many", part, len(part), n_rows, part_outs, part_counts)
 
     def bitmap_to_rows(self, bitmap, n_rows, out_rows, capacity):
         n = c_int64()
-        self._check(self.lib.dr_bitmap_to_rows(self._h, _dp(bitmap), n_rows, _dp(out_rows), capacity, byref(n),
-                                               self._stream()))
+        self._call("dr_bitmap_to_rows", bitmap, n_rows, out_rows, capacity, byref(n))
         return int(n.value)
 
     def bitmap_rows_after_count(self, bitmap, n_rows, out_rows, capacity):
-        self._check(self.lib.dr_bitmap_rows_after_count(self._h, _dp(bitmap), n_rows, _dp(out_rows), capacity,
-                                                        self._stream()))
+        self._call("dr_bitmap_rows_after_count", bitmap, n_rows, out_rows, capacity)
 
     def tile_null_bitmaps(self, tile, n, n_cols, words_per_col, out):
-        self._check(self.lib.dr_tile_null_bitmaps(self._h, _dp(tile), n, n_cols, words_per_col, _dp(out),
-                                                  self._stream()))
+        self._call("dr_tile_null_bitmaps", tile, n, n_cols, words_per_col, out)
 
     def changed_bitmap(self, current, repaired, n, out):
-        self._check(self.lib.dr_changed_bitmap(self._h, _dp(current), _dp(repaired), n, _dp(out), self._stream()))
+        self._call("dr_changed_bitmap", current, repaired, n, out)
 
     def bitmap_gather(self, src, rows, n, out):
-        self._check(self.lib.dr_bitmap_gather(self._h, _dp(src), _dp(rows), n, _dp(out), self._stream()))
+        self._call("dr_bitmap_gather", src, rows, n, out)
 
     def bitmap_clear_rows(self, bitmap, rows, flags, n):
-        self._check(self.lib.dr_bitmap_clear_rows(self._h, _dp(bitmap), _dp(rows), _dp(flags), n, self._stream()))
+        self._call("dr_bitmap_clear_rows", bitmap, rows, flags, n)
 
     # ---- statistics ------------------------------------------------------------------------------
     def discretize(self, vals, n_rows, vmin, denom, thres, out):
-        self._check(self.lib.dr_discretize(self._h, _dp(vals), n_rows, vmin, denom, thres, _dp(out), self._stream()))
+        self._call("dr_discretize", vals, n_rows, vmin, denom, thres, out)
 
     def pair_presence(self, cols, dom, px, py, bit_off, n_rows, block_rows, n_blocks, bits):
-        cp, _k = _ptr_array([c.data_ptr() for c in cols])
-        self._check(self.lib.dr_pair_presence(self._h, cp, _i32_array(dom), len(cols), _i32_array(px), _i32_array(py),
-                                              len(px), _i64_array(bit_off), n_rows, block_rows, n_blocks, _dp(bits),
-                                              self._stream()))
+        self._call("dr_pair_presence", cols, dom, len(cols), px, py, len(px), bit_off, n_rows, block_rows, n_blocks,
+                   bits)
 
     def cooc(self, cols, dom, px, py, tab_off, n_rows, out):
-        cp, _k = _ptr_array([c.data_ptr() for c in cols])
-        self._check(self.lib.dr_cooc(self._h, cp, _i32_array(dom), len(cols), _i32_array(px), _i32_array(py), len(px),
-                                     _i64_array(tab_off), n_rows, _dp(out), self._stream()))
+        self._call("dr_cooc", cols, dom, len(cols), px, py, len(px), tab_off, n_rows, out)
 
     def cooc_skip(self, cols, dom, px, py, tab_off, n_rows, skip, skip_off, out):
         """dr_cooc with one uncounted entry per x value (skip: device int32 or None)."""
-        cp, _k = _ptr_array([c.data_ptr() for c in cols])
-        self._check(self.lib.dr_cooc_skip(self._h, cp, _i32_array(dom), len(cols), _i32_array(px), _i32_array(py),
-                                          len(px), _i64_array(tab_off), n_rows, _dp(skip),
-                                          _i64_array(skip_off) if skip is not None else None, _dp(out),
-                                          self._stream()))
+        self._call("dr_cooc_skip", cols, dom, len(cols), px, py, len(px), tab_off, n_rows, skip,
+                   skip_off if skip is not None else None, out)
 
     def key_presence(self, cols, strides, n_rows, space, bits):
-        cp, _k = _ptr_array([c.data_ptr() for c in cols])
-        self._check(self.lib.dr_key_presence(self._h, cp, _i64_array(strides), len(cols), n_rows, space, _dp(bits),
-                                             self._stream()))
+        self._call("dr_key_presence", cols, strides, len(cols), n_rows, space, bits)
 
     def key_flag(self, cols, strides, n_rows, space, viol_bits, row_bitmap):
-        cp, _k = _ptr_array([c.data_ptr() for c in cols])
-        self._check(self.lib.dr_key_flag(self._h, cp, _i64_array(strides), len(cols), n_rows, space, _dp(viol_bits),
-                                         _dp(row_bitmap), self._stream()))
+        self._call("dr_key_flag", cols, strides, len(cols), n_rows, space, viol_bits, row_bitmap)
 
     def dc_exists(self, left, right, signs, n, group_begin, group_end, out):
-        lp, _k1 = _ptr_array([c.data_ptr() for c in left])
-        rp, _k2 = _ptr_array([c.data_ptr() for c in right])
-        self._check(self.lib.dr_dc_exists(self._h, lp, rp, _i32_array(signs), len(signs), n, _dp(group_begin),
-                                          _dp(group_end), _dp(out), self._stream()))
+        self._call("dr_dc_exists", left, right, signs, len(signs), n, group_begin, group_end, out)
 
     def combine_counts(self, gathered, world, n, seg_off, seg_op, out):
-        self._check(self.lib.dr_combine_counts(self._h, _dp(gathered), world, n, _i64_array(seg_off),
-                                               _i32_array(seg_op), len(seg_op), _dp(out), self._stream()))
+        self._call("dr_combine_counts", gathered, world, n, seg_off, seg_op, len(seg_op), out)
 
     def domain_score(self, rows, n_cells, target, dom_t, corr, dom_c, cooc, hist_t, tau, n_total, beta, out_top1,
                      out_prob, out_weak):
-        cp, _k1 = _ptr_array([c.data_ptr() for c in corr])
-        tp, _k2 = _ptr_array([c.data_ptr() for c in cooc])
-        self._check(self.lib.dr_domain_score(self._h, _dp(rows), n_cells, _dp(target), dom_t, cp, _i32_array(dom_c),
-                                             tp, len(corr), _dp(hist_t), _i64_array(tau), n_total, beta,
-                                             _dp(out_top1), _dp(out_prob), _dp(out_weak), self._stream()))
+        self._call("dr_domain_score", rows, n_cells, target, dom_t, corr, dom_c, cooc, len(corr), hist_t, tau,
+                   n_total, beta, out_top1, out_prob, out_weak)
 
     def domain_prune(self, targets, n_rows, n_total, beta, removed):
         """targets: [(target col, bitmap, hist_t ptr, dom_t, [(corr col, cooc ptr, dom_c, tau)])] -- pointers
         are device addresses (ints) or tensors; removed: device int64[len(targets)], accumulated."""
         arr = (dr_domain_target * max(len(targets), 1))()
-        ptr = lambda x: x if isinstance(x, int) else x.data_ptr()  # noqa: E731
         for i, (tcol, bitmap, hist, dom_t, corr) in enumerate(targets):
             d = arr[i]
-            d.target, d.bitmap, d.hist_t, d.dom_t, d.n_corr = ptr(tcol), ptr(bitmap), ptr(hist), dom_t, len(corr)
+            d.target, d.bitmap, d.hist_t = _address(tcol), _address(bitmap), _address(hist)
+            d.dom_t, d.n_corr = dom_t, len(corr)
             for j, (ccol, cooc, dom_c, tau) in enumerate(corr):
-                d.corr[j], d.cooc[j], d.dom_c[j], d.tau[j] = ptr(ccol), ptr(cooc), dom_c, tau
-        self._check(self.lib.dr_domain_prune(self._h, arr, len(targets), n_rows, n_total, beta, _dp(removed),
-                                             self._stream()))
+                d.corr[j], d.cooc[j], d.dom_c[j], d.tau[j] = _address(ccol), _address(cooc), dom_c, tau
+        self._call("dr_domain_prune", arr, len(targets), n_rows, n_total, beta, removed)
 
     # ---- repair base / tile ----------------------------------------------------------------------
     def gather_rows_masked(self, cols, bitmaps, rows, n, out, f64=False, null_out=None):
         """null_out (int32 codes only): int32 [K][words] that receives the NULL bitmap of every tile column."""
-        cp, _k1 = _ptr_array([c.data_ptr() for c in cols])
-        bp, _k2 = _ptr_array([0 if b is None else b.data_ptr() for b in bitmaps])
         if null_out is not None:
             assert not f64
-            self._check(self.lib.dr_gather_rows_masked_nulls(self._h, cp, bp, len(cols), _dp(rows), n, _dp(out),
-                                                             _dp(null_out), int(null_out.shape[1]), self._stream()))
+            self._call("dr_gather_rows_masked_nulls", cols, bitmaps, len(cols), rows, n, out, null_out,
+                       int(null_out.shape[1]))
             return
-        fn = self.lib.dr_gather_rows_masked_f64 if f64 else self.lib.dr_gather_rows_masked
-        self._check(fn(self._h, cp, bp, len(cols), _dp(rows), n, _dp(out), self._stream()))
+        self._call("dr_gather_rows_masked_f64" if f64 else "dr_gather_rows_masked", cols, bitmaps, len(cols), rows,
+                   n, out)
 
     def tile_null_bitmap(self, tile, n, n_cols, col, out, f64=False):
-        fn = self.lib.dr_tile_null_bitmap_f64 if f64 else self.lib.dr_tile_null_bitmap
-        self._check(fn(self._h, _dp(tile), n, n_cols, col, _dp(out), self._stream()))
+        self._call("dr_tile_null_bitmap_f64" if f64 else "dr_tile_null_bitmap", tile, n, n_cols, col, out)
 
     def gather(self, col, rows, n, out, f64=False):
-        fn = self.lib.dr_gather_f64 if f64 else self.lib.dr_gather_i32
-        self._check(fn(self._h, _dp(col), _dp(rows), n, _dp(out), self._stream()))
+        self._call("dr_gather_f64" if f64 else "dr_gather_i32", col, rows, n, out)
 
     def tile_gather(self, tile, n_cols, col, drows, n, out, f64=False):
-        fn = self.lib.dr_tile_gather_f64 if f64 else self.lib.dr_tile_gather_i32
-        self._check(fn(self._h, _dp(tile), n_cols, col, _dp(drows), n, _dp(out), self._stream()))
+        self._call("dr_tile_gather_f64" if f64 else "dr_tile_gather_i32", tile, n_cols, col, drows, n, out)
 
     def lookup_sorted(self, sorted_rows, n_sorted, keys, n, out):
-        self._check(self.lib.dr_lookup_sorted(self._h, _dp(sorted_rows), n_sorted, _dp(keys), n, _dp(out),
-                                              self._stream()))
+        self._call("dr_lookup_sorted", sorted_rows, n_sorted, keys, n, out)
 
     def forest_predict(self, forest_struct, tile, n_cols, ctile, n_ccols, cells, n_cells, target_col, out_margin=None):
-        self._check(self.lib.dr_forest_predict(self._h, byref(forest_struct), _dp(tile), n_cols, _dp(ctile), n_ccols,
-                                               _dp(cells), n_cells, target_col, _dp(out_margin), self._stream()))
+        self._call("dr_forest_predict", byref(forest_struct), tile, n_cols, ctile, n_ccols, cells, n_cells, target_col,
+                   out_margin)
 
     def forest_predict_ranked(self, forest_struct, tile, n_cols, cells, n_cells, target_col, out_margin=None):
-        self._check(self.lib.dr_forest_predict_ranked(self._h, byref(forest_struct), _dp(tile), n_cols, _dp(cells),
-                                                      n_cells, target_col, _dp(out_margin), self._stream()))
+        self._call("dr_forest_predict_ranked", byref(forest_struct), tile, n_cols, cells, n_cells, target_col,
+                   out_margin)
 
     def gbdt_train(self, params, bins, n_bins, y_class, y_value, weight, init, workspace, out_nodes, out_counts):
-        self._check(self.lib.dr_gbdt_train(
-            self._h, byref(params), _dp(bins), _i32_array(n_bins), _dp(y_class), _dp(y_value), _dp(weight),
-            (c_double * len(init))(*[float(v) for v in init]), _dp(workspace), workspace.numel(), _dp(out_nodes),
-            _dp(out_counts), self._stream()))
+        self._call("dr_gbdt_train", byref(params), bins, n_bins, y_class, y_value, weight,
+                   (c_double * len(init))(*[float(v) for v in init]), workspace, workspace.numel(), out_nodes,
+                   out_counts)
 
     def gbdt_workspace_bytes(self, n_rows, n_seq):
         return int(self.lib.dr_gbdt_workspace_bytes(n_rows, n_seq))
 
     def tile_fill(self, tile, n_cols, col, cells, n_cells, value):
-        self._check(self.lib.dr_tile_fill_i32(self._h, _dp(tile), n_cols, col, _dp(cells), n_cells, value,
-                                              self._stream()))
+        self._call("dr_tile_fill_i32", tile, n_cols, col, cells, n_cells, value)
 
     def scatter(self, col, rows, vals, n, f64=False):
-        fn = self.lib.dr_scatter_f64 if f64 else self.lib.dr_scatter_i32
-        self._check(fn(self._h, _dp(col), _dp(rows), _dp(vals), n, self._stream()))
+        self._call("dr_scatter_f64" if f64 else "dr_scatter_i32", col, rows, vals, n)
 
     def fd_map_build(self, x_col, x_mask, y_col, y_mask, n_rows, dom_x, lo, hi):
-        self._check(self.lib.dr_fd_map_build(self._h, _dp(x_col), _dp(x_mask), _dp(y_col), _dp(y_mask), n_rows,
-                                             dom_x, _dp(lo), _dp(hi), self._stream()))
+        self._call("dr_fd_map_build", x_col, x_mask, y_col, y_mask, n_rows, dom_x, lo, hi)
 
     def tile_lut_fill(self, tile, n_cols, x_col, y_col, cells, n_cells, lut, lut_size):
-        self._check(self.lib.dr_tile_lut_fill(self._h, _dp(tile), n_cols, x_col, y_col, _dp(cells), n_cells,
-                                              _dp(lut), lut_size, self._stream()))
+        self._call("dr_tile_lut_fill", tile, n_cols, x_col, y_col, cells, n_cells, lut, lut_size)
 
     # ---- delphi.misc ------------------------------------------------------------------------------
     def kmeans_assign(self, cols, dom, p_off, n_rows, P, mu_sq, labels, split=None):
         """One k-means assignment over dictionary codes: P device float64 [p_rows][n_centres], mu_sq device
         float64 [n_centres]; labels device int32, written in place (only rows split[label] >= 0 with split)."""
-        cp, _k = _ptr_array([c.data_ptr() for c in cols])
-        self._check(self.lib.dr_kmeans_assign(
-            self._h, cp, _i32_array(dom), _i64_array(p_off), len(cols), n_rows, _dp(P), int(P.shape[0]), _dp(mu_sq),
-            int(P.shape[1]), _dp(split), 0 if split is None else int(split.numel()), _dp(labels), self._stream()))
+        self._call("dr_kmeans_assign", cols, dom, p_off, len(cols), n_rows, P, int(P.shape[0]), mu_sq,
+                   int(P.shape[1]), split, 0 if split is None else int(split.numel()), labels)
 
     def label_counts(self, labels, col, dom, n_rows, lab_lo, lab_hi, out):
         """out (device int64 [lab_hi - lab_lo][dom + 1], zeroed) += counts of (label, code slot)."""
-        self._check(self.lib.dr_label_counts(self._h, _dp(labels), _dp(col), dom, n_rows, lab_lo, lab_hi, _dp(out),
-                                             self._stream()))
+        self._call("dr_label_counts", labels, col, dom, n_rows, lab_lo, lab_hi, out)
 
     def error_map(self, bitmaps, n_rows, out):
-        bp, _k = _ptr_array([0 if b is None else b.data_ptr() for b in bitmaps])
-        self._check(self.lib.dr_error_map(self._h, bp, len(bitmaps), n_rows, _dp(out), self._stream()))
+        self._call("dr_error_map", bitmaps, len(bitmaps), n_rows, out)
 
     def null_bits(self, valid, bit_offset, n_rows, row_base, key, ratio, out):
-        self._check(self.lib.dr_null_bits(self._h, _dp(valid), bit_offset, n_rows, row_base, key & ((1 << 64) - 1),
-                                          float(ratio), _dp(out), self._stream()))
+        self._call("dr_null_bits", valid, bit_offset, n_rows, row_base, key & ((1 << 64) - 1), float(ratio), out)
 
     def flatten(self, cols, base, n_rows, row_ids, out_codes, out_valid, out_ids):
-        cp, _k = _ptr_array([c.data_ptr() for c in cols])
-        self._check(self.lib.dr_flatten(self._h, cp, _i64_array(base), len(cols), n_rows, _dp(row_ids),
-                                        _dp(out_codes), _dp(out_valid), _dp(out_ids), self._stream()))
+        self._call("dr_flatten", cols, base, len(cols), n_rows, row_ids, out_codes, out_valid, out_ids)
 
 
 def _profiled(name, fn):
+    @functools.wraps(fn)
     def wrapper(self, *args, **kwargs):
         if self.profile is None:
             return fn(self, *args, **kwargs)
@@ -586,18 +531,14 @@ def _profiled(name, fn):
         finally:
             end.record()
             self.profile.append((name, start, end))
-    wrapper.__name__ = name
     return wrapper
 
 
-for _name in ("widen_u8", "h2d_copy", "d2h_copy", "index_presence", "index_remap", "ids_unique", "gather_i64", "valid_bits",
-              "scan_hist", "lut_scan", "quartiles", "range_flag", "dc_const", "dc_fd_build", "dc_fd_flag", "bitmap_or",
-              "bitmap_andnot", "bitmap_count", "bitmap_count_many", "bitmap_to_rows_async", "bitmaps_to_rows_many", "bitmap_to_rows", "bitmap_rows_after_count", "tile_null_bitmaps", "changed_bitmap", "bitmap_gather", "bitmap_clear_rows", "discretize",
-              "pair_presence", "cooc", "cooc_skip", "key_presence", "key_flag", "dc_exists", "combine_counts", "dc_lt_flag",
-              "dc_hash_build", "dc_hash_flag", "domain_score", "domain_prune", "gather_rows_masked", "tile_null_bitmap", "gather",
-              "tile_gather", "lookup_sorted", "forest_predict", "forest_predict_ranked", "tile_fill", "gbdt_train",
-              "kmeans_assign", "label_counts", "error_map", "null_bits", "flatten"):
-    setattr(Context, _name, _profiled(_name, getattr(Context, _name)))
+# The public methods that do no device work; every other one records one profile entry per call, under its name.
+_NOT_PROFILED = {"close", "acquire", "release", "launch_count", "gbdt_workspace_bytes"}
+for _name, _fn in list(vars(Context).items()):
+    if not _name.startswith("_") and _name not in _NOT_PROFILED:
+        setattr(Context, _name, _profiled(_name, _fn))
 
 
 def profile_summary(ctx):

@@ -33,6 +33,63 @@ def test_library_exports_every_declared_symbol():
         getattr(raw, sym)
 
 
+def _declarations():
+    """{name: (return type, [parameter declarations])} of every function the header declares."""
+    hdr = open(os.path.join(ROOT, "include", "b200repair.h")).read()
+    hdr = re.sub(r"/\*.*?\*/", "", hdr, flags=re.S)
+    hdr = re.sub(r"^\s*#.*$", "", hdr, flags=re.M)
+    out = {}
+    for stmt in hdr.split(";"):
+        m = re.match(r"\s*(.+?)\b(dr_\w+)\s*\((.*)\)\s*$", stmt, flags=re.S)
+        if m:
+            params = [p.strip() for p in m.group(3).split(",")]
+            out[m.group(2)] = (m.group(1).strip(), [] if params == ["void"] else params)
+    return out
+
+
+_C_KINDS = {"int": "i32", "int32_t": "i32", "uint32_t": "i32", "int64_t": "i64", "uint64_t": "i64", "double": "f64"}
+
+
+def _c_kind(decl):
+    """ptr, i32, i64 or f64 of a C type, or of a parameter declaration (type then name)."""
+    return "ptr" if "*" in decl else _C_KINDS[decl.split()[0]]
+
+
+def _ctypes_kind(t):
+    if issubclass(t, (ctypes._Pointer, ctypes.c_void_p, ctypes.c_char_p)):
+        return "ptr"
+    if t._type_ == "d":
+        return "f64"
+    assert t._type_ in "iIlLqQ", t
+    return "i%d" % (8 * ctypes.sizeof(t))
+
+
+def test_binding_signatures_match_the_header():
+    """Every _SIGNATURES row has the header's parameter count and, per position, the same kind: a ctypes
+    integer of the wrong width would be truncated or misread silently."""
+    from repair import _native
+    decls = _declarations()
+    assert sorted(decls) == _declared_symbols()
+    assert sorted(_native._SIGNATURES) == sorted(decls)
+    for name, (ret, params) in decls.items():
+        restype, argtypes = _native._SIGNATURES[name]
+        assert _ctypes_kind(restype) == _c_kind(ret), name
+        assert [_ctypes_kind(t) for t in argtypes] == [_c_kind(p) for p in params], name
+
+
+def test_every_device_call_is_profiled():
+    """bench.py's per-kernel table is built from the profile: every public Context method that can do device
+    work must record itself."""
+    from repair import _native
+    no_device_work = {"close", "acquire", "release", "launch_count", "gbdt_workspace_bytes"}
+    public = {n: f for n, f in vars(_native.Context).items() if not n.startswith("_")}
+    assert no_device_work <= set(public)
+    profiled_code = _native._profiled("probe", lambda self: None).__code__
+    unprofiled = sorted(n for n, f in public.items()
+                        if n not in no_device_work and getattr(f, "__code__", None) is not profiled_code)
+    assert unprofiled == []
+
+
 def test_engine_fails_loudly_without_cuda():
     import torch
     if torch.cuda.is_available():
