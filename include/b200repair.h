@@ -493,6 +493,41 @@ int dr_gbdt_train(dr_ctx* ctx, const dr_gbdt_params* params, const uint8_t* bins
                   const int32_t* y_class, const double* y_value, const double* weight, const double* init,
                   void* workspace, int64_t workspace_bytes, dr_gbdt_node* out_nodes, int32_t* out_counts,
                   void* stream);
+/* dr_gbdt_train_ex: dr_gbdt_train with the boosting options model.lgb.boosting_type, reg_alpha and
+ * min_split_gain (train.py:102-115), specified in oracle/gbdt_boost.py and reproduced bit for bit.
+ * boost == NULL, or gbdt with reg_alpha = min_split_gain = 0, is exactly dr_gbdt_train (same launches,
+ * same workspace); otherwise the workspace is dr_gbdt_train_ex_workspace_bytes(n_rows, S, drop_off[n_iter])
+ * bytes (n_drops = 0 unless dart).
+ *   reg_alpha       L1: gains and leaves use T(G) = sign(G) * max(|G| - reg_alpha * qscale, 0) for G
+ *   min_split_gain  a leaf splits only when its best gain > min_split_gain * qscale
+ *   goss            iterations >= goss_warmup keep the goss_top_k rows of largest sum_k |g * h| (ties
+ *                   included) and each other row iff hash(seed, iteration, row) < other_k / (n - top_k),
+ *                   its g and h multiplied by (n - top_k) / other_k before quantisation; the caller
+ *                   divides qscale by 2^ceil(log2 of that factor) so that bins still fit int32.  Row
+ *                   bagging (subsample / subsample_freq) is ignored.
+ *   rf              gradients of the initial scores only; bags and feature subsets per iteration as
+ *                   gbdt; leaf values divided by n_iter instead of scaled by the learning rate.  Needs
+ *                   row bagging or colsample_bytree < 1 (DR_ERR_INVALID otherwise).
+ *   dart            iteration it first subtracts the trees of iterations drop_iter[drop_off[it] ..
+ *                   drop_off[it + 1]) (ascending, all < it) from the scores, grows its trees with
+ *                   learning_rate / (1 + k), then multiplies the dropped trees' leaves in out_nodes by
+ *                   k / (k + 1) and adds them back.  The schedule is the caller's (host arrays). */
+#define DR_GBDT_BOOST_GBDT 0
+#define DR_GBDT_BOOST_DART 1
+#define DR_GBDT_BOOST_GOSS 2
+#define DR_GBDT_BOOST_RF 3
+typedef struct dr_gbdt_boost {
+    int32_t boosting;                        /* DR_GBDT_BOOST_* */
+    int32_t goss_warmup, goss_top_k, goss_other_k;
+    double reg_alpha, min_split_gain;
+    const int32_t* drop_off;                 /* dart: host int32[n_iter + 1], drop_off[0] = 0 */
+    const int32_t* drop_iter;                /* dart: host int32[drop_off[n_iter]] */
+} dr_gbdt_boost;
+int64_t dr_gbdt_train_ex_workspace_bytes(int32_t n_rows, int32_t n_seq, int64_t n_drops);
+int dr_gbdt_train_ex(dr_ctx* ctx, const dr_gbdt_params* params, const dr_gbdt_boost* boost, const uint8_t* bins,
+                     const int32_t* n_bins, const int32_t* y_class, const double* y_value, const double* weight,
+                     const double* init, void* workspace, int64_t workspace_bytes, dr_gbdt_node* out_nodes,
+                     int32_t* out_counts, void* stream);
 
 /* ---- 8f #4: rule-based repairs -----------------------------------------------------------------
  * dr_scatter_*: col[rows[i]] = vals[i] -- repairs decided by a rule join the repair base

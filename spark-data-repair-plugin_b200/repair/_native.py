@@ -60,6 +60,14 @@ class dr_gbdt_params(ctypes.Structure):
                 ("subsample_freq", c_int32), ("seed", c_int32)]
 
 
+class dr_gbdt_boost(ctypes.Structure):
+    _fields_ = [("boosting", c_int32), ("goss_warmup", c_int32), ("goss_top_k", c_int32), ("goss_other_k", c_int32),
+                ("reg_alpha", c_double), ("min_split_gain", c_double), ("drop_off", c_void_p), ("drop_iter", c_void_p)]
+
+
+DR_GBDT_BOOST = {"gbdt": 0, "dart": 1, "goss": 2, "rf": 3}
+
+
 # ---- argument kinds --------------------------------------------------------------------------------
 # Pointer-width ctypes types whose from_param converts a Python value at call time.  ctypes keeps what
 # from_param returns alive until the C function returns, so the host arrays built here need no other
@@ -175,6 +183,9 @@ _SIGNATURES = {
     "dr_gbdt_workspace_bytes": (c_int64, [c_int32, c_int32]),
     "dr_gbdt_train": (c_int, [c_void_p, POINTER(dr_gbdt_params), _Buf, _I32s, _Buf, _Buf, _Buf, POINTER(c_double),
                               _Buf, c_int64, _Buf, _Buf, c_void_p]),
+    "dr_gbdt_train_ex_workspace_bytes": (c_int64, [c_int32, c_int32, c_int64]),
+    "dr_gbdt_train_ex": (c_int, [c_void_p, POINTER(dr_gbdt_params), POINTER(dr_gbdt_boost), _Buf, _I32s, _Buf, _Buf,
+                                 _Buf, POINTER(c_double), _Buf, c_int64, _Buf, _Buf, c_void_p]),
     "dr_tile_fill_i32": (c_int, [c_void_p, _Buf, c_int, c_int, _Buf, c_int64, c_int32, c_void_p]),
     "dr_scatter_i32": (c_int, [c_void_p, _Buf, _Buf, _Buf, c_int64, c_void_p]),
     "dr_scatter_f64": (c_int, [c_void_p, _Buf, _Buf, _Buf, c_int64, c_void_p]),
@@ -484,6 +495,17 @@ class Context:
 
     def gbdt_workspace_bytes(self, n_rows, n_seq):
         return int(self.lib.dr_gbdt_workspace_bytes(n_rows, n_seq))
+
+    def gbdt_train_ex(self, params, boost, bins, n_bins, y_class, y_value, weight, init, workspace, out_nodes,
+                      out_counts):
+        """dr_gbdt_train with boosting options: boost is a dr_gbdt_boost (its drop schedule arrays must stay
+        alive for the call) or None."""
+        self._call("dr_gbdt_train_ex", byref(params), None if boost is None else byref(boost), bins, n_bins, y_class,
+                   y_value, weight, (c_double * len(init))(*[float(v) for v in init]), workspace, workspace.numel(),
+                   out_nodes, out_counts)
+
+    def gbdt_train_ex_workspace_bytes(self, n_rows, n_seq, n_drops):
+        return int(self.lib.dr_gbdt_train_ex_workspace_bytes(n_rows, n_seq, n_drops))
 
     def tile_fill(self, tile, n_cols, col, cells, n_cells, value):
         self._call("dr_tile_fill_i32", tile, n_cols, col, cells, n_cells, value)

@@ -3,9 +3,12 @@ sample, computes class weights / initial scores, runs the whole boosting loop on
 flattens the result into the exchange format of ``forest.py``.
 
 Eligibility: every feature discrete (label-encoded attribute behind a sum / ordinal encoder) and at
-most 128 encoded features; a feature with more than 254 distinct encoded values is binned like
-LightGBM's max_bin does (adjacent values share a bin).  Other models (continuous features) use
-``train.build_model`` (scikit-learn)."""
+most 128 encoded features; a feature with more than max_bin - 1 distinct encoded values (254 at the
+default max_bin = 255) is binned like LightGBM's max_bin does (adjacent values share a bin).  Other
+models (continuous features) use ``train.build_model`` (scikit-learn).
+
+Boosting options (``model.lgb.boosting_type`` dart / goss / rf, ``reg_alpha``, ``min_split_gain``) run
+through ``dr_gbdt_train_ex``; at their defaults the trainer is called exactly as before."""
 import numpy as np
 
 from .forest import encoder_lut
@@ -22,8 +25,10 @@ def quant_bits(n_rows):
     return int(min(24, 30 - int(np.ceil(np.log2(max(n_rows, 2))))))
 
 
-def bin_sample(encoders, sample_codes, dict_sizes):
-    """-> (bins uint8 [n, F'], n_bins int32 [F'], bin_values list of float arrays) or None."""
+def bin_sample(encoders, sample_codes, dict_sizes, max_bin=255):
+    """-> (bins uint8 [n, F'], n_bins int32 [F'], bin_values list of float arrays) or None.
+    A feature gets at most max_bin - 1 value bins (max_bin clamped to [2, 255]) plus the missing bin."""
+    max_real = min(255, max(2, int(max_bin))) - 1
     cols, n_bins, values = [], [], []
     for e in encoders:
         if e["type"] == "cont":
@@ -34,13 +39,13 @@ def bin_sample(encoders, sample_codes, dict_sizes):
             col = lut[:, j]
             vals = np.unique(col[~np.isnan(col)])
             ok = ~np.isnan(col)
-            if len(vals) > MAX_BINS:
+            if len(vals) > max_real:
                 # more distinct values than bins (LightGBM: max_bin = 255, train.py:106): adjacent values
                 # share a bin, bins of about equal sample counts; thresholds only fall between bins
                 enc = col[codes + 1]
                 cnt = np.bincount(np.searchsorted(vals, enc[~np.isnan(enc)]), minlength=len(vals)).astype(np.float64)
-                edge = np.floor(np.cumsum(cnt) / max(cnt.sum(), 1.0) * MAX_BINS - 1e-9).astype(np.int64)
-                group = np.minimum(np.maximum.accumulate(np.clip(edge, 0, MAX_BINS - 1)), MAX_BINS - 1)
+                edge = np.floor(np.cumsum(cnt) / max(cnt.sum(), 1.0) * max_real - 1e-9).astype(np.int64)
+                group = np.minimum(np.maximum.accumulate(np.clip(edge, 0, max_real - 1)), max_real - 1)
                 _, group = np.unique(group, return_inverse=True)      # dense bin ids, in value order
                 n_real = int(group.max()) + 1
                 upper = np.array([vals[group == b].max() for b in range(n_real)])
@@ -82,12 +87,69 @@ def initial_scores(y, n_classes, weight):
     return np.zeros(n_classes)
 
 
+def _h24(key):
+    """Top 24 bits of the splitmix64 finaliser of key (the trainer's hash)."""
+    z = key & _M64
+    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & _M64
+    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & _M64
+    return (z ^ (z >> 31)) >> 40
+
+
+_M64 = (1 << 64) - 1
+_GOLDEN = 0x9E3779B97F4A7C15
+
+
+def dart_schedule(n_iter, learning_rate, seed, drop_rate=0.1, max_drop=50, skip_drop=0.5):
+    """DART's drop schedule -> (drop_off int32 [n_iter + 1], drop_iter int32): iteration it drops the earlier
+    iterations drop_iter[drop_off[it]:drop_off[it + 1]].  LightGBM's non-uniform rule over tree weights:
+    an iteration skips dropping with probability skip_drop; otherwise tree i goes with probability
+    rate * w_i * T / W (T trees of total weight W, rate = min(drop_rate, max_drop * T / W^2)), at most
+    max_drop of them; a new tree weighs learning_rate / (1 + k), dropped ones shrink by k / (k + 1)."""
+    unit = float(1 << 24)
+    weights, total = [], 0.0
+    off, flat = [0], []
+    for it in range(n_iter):
+        k = 0
+        if it > 0 and _h24((seed + 4) * _GOLDEN + it) / unit >= skip_drop:
+            inv_avg = float(it) / total
+            rate = min(drop_rate, max_drop * inv_avg / total) if max_drop > 0 else drop_rate
+            for i in range(it):
+                if _h24((seed + 3) * _GOLDEN + (it << 32) + i) / unit < rate * weights[i] * inv_avg:
+                    flat.append(i)
+                    k += 1
+                    if k == max_drop:
+                        break
+        for i in flat[len(flat) - k:]:
+            total -= weights[i] * (1.0 / (k + 1.0))
+            weights[i] *= k / (k + 1.0)
+        weights.append(learning_rate / (1.0 + k))
+        total += weights[-1]
+        off.append(len(flat))
+    return np.asarray(off, dtype=np.int32), np.asarray(flat, dtype=np.int32)
+
+
+def goss_counts(n, top_rate=0.2, other_rate=0.1):
+    """-> (top_k, other_k, quantisation shift): GOSS keeps the top_k rows by |g * h| and draws the others
+    with probability other_k / (n - top_k), amplified by m = (n - top_k) / other_k; qscale is divided by
+    2^ceil(log2 m) so that histogram bins keep fitting int32."""
+    top_k, other_k = max(1, int(n * top_rate)), int(n * other_rate)
+    m = (n - top_k) / other_k if other_k > 0 else 1.0
+    shift = 0
+    while float(1 << shift) < m:
+        shift += 1
+    return top_k, other_k, shift
+
+
 def train_gpu(ctx, device, bins, n_bins, bin_values, y, n_classes, weight, n_iter, learning_rate, max_depth,
               num_leaves=31, min_data_in_leaf=20, min_sum_hessian=1e-3, reg_lambda=0.0, colsample_bytree=1.0,
-              subsample=1.0, subsample_freq=0, seed=42):
-    """-> flat forest (forest.py layout)."""
+              subsample=1.0, subsample_freq=0, seed=42, boosting="gbdt", reg_alpha=0.0, min_split_gain=0.0,
+              top_rate=0.2, other_rate=0.1, drop_rate=0.1, max_drop=50, skip_drop=0.5):
+    """-> flat forest (forest.py layout).  boosting / reg_alpha / min_split_gain away from their defaults
+    select dr_gbdt_train_ex (top_rate / other_rate: goss, drop_rate / max_drop / skip_drop: dart)."""
     import torch
-    from ._native import dr_gbdt_params
+    from ._native import DR_GBDT_BOOST, dr_gbdt_boost, dr_gbdt_params
+    if boosting not in DR_GBDT_BOOST:
+        raise ValueError("boosting must be one of {}".format(sorted(DR_GBDT_BOOST)))
     n, F = bins.shape
     S = 1 if n_classes <= 2 else n_classes
     init = initial_scores(y, n_classes, weight)
@@ -96,6 +158,16 @@ def train_gpu(ctx, device, bins, n_bins, bin_values, y, n_classes, weight, n_ite
         qscale = float(2 ** quant_bits(n)) / max(float(np.abs(yv - init[0]).max()), 1e-300)
     else:
         qscale = float(2 ** quant_bits(n)) / float(np.max(weight))
+    boost = None
+    if boosting != "gbdt" or reg_alpha != 0.0 or min_split_gain != 0.0:
+        boost = dr_gbdt_boost(DR_GBDT_BOOST[boosting], 0, 0, 0, float(reg_alpha), float(min_split_gain), None, None)
+        if boosting == "goss":
+            top_k, other_k, shift = goss_counts(n, top_rate, other_rate)
+            boost.goss_warmup, boost.goss_top_k, boost.goss_other_k = int(1.0 / learning_rate), top_k, other_k
+            qscale = qscale / float(1 << shift)
+        if boosting == "dart":
+            drop_off, drop_iter = dart_schedule(n_iter, learning_rate, seed, drop_rate, max_drop, skip_drop)
+            boost.drop_off, boost.drop_iter = drop_off.ctypes.data, drop_iter.ctypes.data
     prm = dr_gbdt_params(n, F, n_classes, n_iter, max_depth, num_leaves, min_data_in_leaf, learning_rate,
                          min_sum_hessian, qscale, float(reg_lambda), float(colsample_bytree), float(subsample),
                          int(subsample_freq), int(seed))
@@ -103,10 +175,15 @@ def train_gpu(ctx, device, bins, n_bins, bin_values, y, n_classes, weight, n_ite
     d_yc = torch.from_numpy(np.ascontiguousarray(y, dtype=np.int32)).to(device) if n_classes >= 2 else None
     d_yv = torch.from_numpy(np.ascontiguousarray(y, dtype=np.float64)).to(device) if n_classes == 1 else None
     d_w = torch.from_numpy(np.ascontiguousarray(weight, dtype=np.float64)).to(device)
-    ws = torch.empty(ctx.gbdt_workspace_bytes(n, S), dtype=torch.uint8, device=device)
     out_nodes = torch.zeros(n_iter * S * MAX_NODES * NODE_DTYPE.itemsize, dtype=torch.uint8, device=device)
     out_counts = torch.zeros(n_iter * S, dtype=torch.int32, device=device)
-    ctx.gbdt_train(prm, d_bins, n_bins, d_yc, d_yv, d_w, init, ws, out_nodes, out_counts)
+    if boost is None:
+        ws = torch.empty(ctx.gbdt_workspace_bytes(n, S), dtype=torch.uint8, device=device)
+        ctx.gbdt_train(prm, d_bins, n_bins, d_yc, d_yv, d_w, init, ws, out_nodes, out_counts)
+    else:
+        n_drops = int(drop_off[-1]) if boosting == "dart" else 0
+        ws = torch.empty(ctx.gbdt_train_ex_workspace_bytes(n, S, n_drops), dtype=torch.uint8, device=device)
+        ctx.gbdt_train_ex(prm, boost, d_bins, n_bins, d_yc, d_yv, d_w, init, ws, out_nodes, out_counts)
     nodes = out_nodes.cpu().numpy().view(NODE_DTYPE).reshape(n_iter, S, MAX_NODES)
     counts = out_counts.cpu().numpy().reshape(n_iter, S)
     return flatten(nodes, counts, init, bin_values, F, n_classes)

@@ -459,8 +459,10 @@ def _fit(rm, engine, encoders, codes, tile_col, features, dict_sizes, X, y_value
     from . import search as HS
     from .train import _get, search_options
     binned = None
+    boosting = _get(rm.opts, "model.lgb.boosting_type")
     if rm.trainer != "sklearn" and is_discrete:
-        binned = G.bin_sample(encoders, {f: codes[:, tile_col[f]] for f in features}, dict_sizes)
+        binned = G.bin_sample(encoders, {f: codes[:, tile_col[f]] for f in features}, dict_sizes,
+                              max_bin=_get(rm.opts, "model.lgb.max_bin"))
     if binned is not None and int(binned[1].sum()) * 12 <= 200 * 1024:
         bins, n_bins, values = binned
         classes = sorted(set(int(v) for v in y_values.tolist()))
@@ -479,10 +481,13 @@ def _fit(rm, engine, encoders, codes, tile_col, features, dict_sizes, X, y_value
                                min_sum_hessian=float(params["min_child_weight"]),
                                reg_lambda=float(params["reg_lambda"]),
                                colsample_bytree=float(params["colsample_bytree"]),
-                               subsample=float(params["subsample"]), subsample_freq=int(params["subsample_freq"]))
+                               subsample=float(params["subsample"]), subsample_freq=int(params["subsample_freq"]),
+                               boosting=boosting, reg_alpha=_get(rm.opts, "model.lgb.reg_alpha"),
+                               min_split_gain=_get(rm.opts, "model.lgb.min_split_gain"))
 
         max_evals, no_progress, timeout, n_splits = search_options(rm.opts)
-        params = dict(HS.DEFAULTS)
+        defaults = HS.RF_DEFAULTS if boosting == "rf" else HS.DEFAULTS
+        params = dict(defaults)
         if max_evals > 1 and y is not None:
             folds = HS.cv_folds(y_idx, True, n_splits)
             tile = engine.torch.from_numpy(np.ascontiguousarray(codes, dtype=np.int32)).to(engine.device)
@@ -500,7 +505,7 @@ def _fit(rm, engine, encoders, codes, tile_col, features, dict_sizes, X, y_value
                     scores.append(HS.score(y_values[va], pred, True))
                 return -float(np.mean(scores)), [-float(v) for v in scores]
 
-            params, _, n_eval = HS.search(evaluate, max_evals, no_progress, timeout)
+            params, _, n_eval = HS.search(evaluate, max_evals, no_progress, timeout, defaults=defaults)
             rm.last_run.setdefault("search", {})[y] = {"evals": n_eval, "params": params}
         return {"forest": train(params), "class_codes": classes}
     forest, classes = build_model(X, y_values, is_discrete, num_class, rm.opts)

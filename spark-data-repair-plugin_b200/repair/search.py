@@ -123,26 +123,32 @@ def score(y_true, y_pred, is_discrete):
     return -float(np.mean(d * d))
 
 
-def search(evaluate, max_evals, no_progress_loss, timeout, seed=42):
+# trial 0 under boosting_type rf: LightGBM refuses rf without row bagging or feature sub-sampling, so the
+# defaults draw a new bag per tree at the bootstrap's expected share of distinct rows
+RF_DEFAULTS = dict(DEFAULTS, subsample=0.632, subsample_freq=1)
+
+
+def search(evaluate, max_evals, no_progress_loss, timeout, seed=42, defaults=None):
     """``fmin`` of train.py:198-209.  evaluate(params) -> loss (= -mean CV score; exceptions count as
     0.0 like train.py:176-180), or (loss, per-fold losses).  -> (best params, best loss, number of
-    evaluations).
+    evaluations).  defaults: trial 0 and the ``max_evals <= 1`` result (LightGBM's ``DEFAULTS`` if None).
 
     One deliberate deviation from hyperopt's plain argmin: k-fold CV on a few hundred rows is noisy, so a
     tuned configuration only replaces LightGBM's defaults (trial 0) when it beats them by more than one
     standard error of the defaults' own fold losses (the "one-standard-error rule" of model selection).
     Without it a short search degrades heavy-tailed regression targets (boston CRIM: 8 % better CV MSE,
     12 % worse RMSE on the repaired cells) while helping others (TAX: 23 % better CV MSE, 24 % better RMSE)."""
+    defaults = DEFAULTS if defaults is None else defaults
     if max_evals <= 1:
-        return dict(DEFAULTS), None, 0
+        return dict(defaults), None, 0
     rng = np.random.default_rng(seed)
     trials = []          # (vector in search space, loss)
-    best_loss, best_params, since_best = None, dict(DEFAULTS), 0
+    best_loss, best_params, since_best = None, dict(defaults), 0
     default_loss, default_se = None, 0.0
     t0 = time.time()
     for it in range(int(min(max_evals, 1 << 30))):
         if it == 0:
-            params, vec = dict(DEFAULTS), None
+            params, vec = dict(defaults), None
         else:
             vec = _draw_prior(rng) if len(trials) < N_STARTUP else _suggest(rng, trials)
             params = _to_params(vec)
@@ -168,6 +174,6 @@ def search(evaluate, max_evals, no_progress_loss, timeout, seed=42):
         if since_best >= no_progress_loss or (timeout > 0 and time.time() - t0 > timeout):
             break
     if default_loss is not None and best_loss is not None and not best_loss < default_loss - default_se:
-        best_params, best_loss = dict(DEFAULTS), default_loss     # not a significant improvement
+        best_params, best_loss = dict(defaults), default_loss     # not a significant improvement
     _logger.info("hyperopt: #eval={}/{}".format(it + 1, max_evals))
     return best_params, best_loss, it + 1

@@ -105,6 +105,10 @@ def sklearn_estimator(is_discrete, opts, params):
     return HistGradientBoostingRegressor(**common)
 
 
+# model.lgb.* options scikit-learn's histogram GBDT has no counterpart for, with their defaults
+_GPU_ONLY_OPTS = (("model.lgb.boosting_type", "gbdt"), ("model.lgb.reg_alpha", 0.0), ("model.lgb.min_split_gain", 0.0))
+
+
 def build_model(X, y, is_discrete, num_class, opts):
     """-> (flat forest, class labels ascending or None) or (None, None) when training fails
     (the reference swallows failures into PoorModel(None), train.py:227-229).
@@ -112,6 +116,11 @@ def build_model(X, y, is_discrete, num_class, opts):
     Fixed parameters follow train.py:102-115; the seven tuned parameters come from the search of
     search.py (train.py:133-229) -- LightGBM's defaults when ``model.hp.max_evals`` is 1."""
     from . import search as HS
+    ignored = ["{}={}".format(k, _get(opts, k)) for k, d in _GPU_ONLY_OPTS if _get(opts, k) != d]
+    if ignored:
+        _logger.warning("{} has no effect on this model: it is trained by scikit-learn's histogram GBDT "
+                        "(continuous target or features), which has no dart, goss, rf, L1 or gain floor"
+                        .format(", ".join(ignored)))
     try:
         X = np.asarray(X, dtype=np.float64)
         if X.shape[1] == 0:
