@@ -381,7 +381,11 @@ int dr_lookup_sorted(dr_ctx* ctx, const int32_t* sorted, int64_t n_sorted, const
  *                        ties -> lowest s; written to tile[row][target_col]
  *   kind 1 (regressor)   value (rounded half-to-even like numpy.round when `integral`) written
  *                        to ctile[row][target_ccol]
- * out_margin (optional, device double[n_cells * n_seq]) receives the margins (pmf modes). */
+ * out_margin (optional, device double[n_cells * n_seq]) receives the margins (pmf modes).
+ * Precondition: when any feat_col[f] < 0 (a continuous feature), ctile must be a device double
+ *   [rows][n_ccols] with n_ccols > -feat_col[f] - 1.  feat_col lives in device memory, so this entry
+ *   point cannot check it; only a regressor's own ctile / target column are validated here.  Callers
+ *   check it on the host (repair/forest.py DeviceModel.predict). */
 typedef struct dr_forest {
     int32_t n_seq, n_trees, n_nodes, n_feat;
     const int32_t* seq_tree_off;

@@ -426,6 +426,8 @@ class DeviceModel:
                 luts.append(lut[:, j])
                 lut_off.append(lut_off[-1] + lut.shape[0])
         n_feat = len(feat_col)
+        # largest float64-tile column a walk reads (-1: none); predict() checks the tile it is given covers it
+        self.max_ccol = max([-c - 1 for c in feat_col if c < 0], default=-1)
         if n_feat != int(f["n_features"]):
             raise ValueError("encoder layout ({} features) does not match the forest ({})".format(
                 n_feat, int(f["n_features"])))
@@ -502,7 +504,13 @@ class DeviceModel:
     def predict(self, ctx, tile, n_cols, ctile, n_ccols, cells, n_cells, target_col, out_margin=None,
                 force_generic=False):
         """Fills the target column of the listed tile rows in place (rank-coded kernel when the model
-        qualifies, the generic float64 kernel otherwise)."""
+        qualifies, the generic float64 kernel otherwise).  A model with a continuous feature or target needs
+        the float64 tile (ctile, n_ccols columns): the kernel reads it without a check of its own."""
+        if self.max_ccol >= 0 and (ctile is None or n_ccols <= self.max_ccol):
+            raise ValueError("the model reads float64 tile column {} but got {}".format(
+                self.max_ccol, "no float64 tile" if ctile is None else "{} columns".format(n_ccols)))
+        if self.kind == 1 and ctile is None:
+            raise ValueError("a regressor writes its predictions to the float64 tile, but got none")
         if self.ranked is not None and not force_generic:
             ctx.forest_predict_ranked(self.ranked, tile, n_cols, cells, n_cells, target_col, out_margin)
         else:

@@ -2,13 +2,16 @@
 sample, computes class weights / initial scores, runs the whole boosting loop on the device and
 flattens the result into the exchange format of ``forest.py``.
 
-Eligibility: every feature discrete (label-encoded attribute behind a sum / ordinal encoder) and at
-most 128 encoded features; a feature with more than max_bin - 1 distinct encoded values (254 at the
-default max_bin = 255) is binned like LightGBM's max_bin does (adjacent values share a bin).  Other
-models (continuous features) use ``train.build_model`` (scikit-learn).
+Eligibility: at most 128 encoded features; a feature with more than max_bin - 1 distinct values (254 at
+the default max_bin = 255) is binned like LightGBM's max_bin does (adjacent values share a bin).  Which
+models come here is decided by ``model.gpu_trainer_bins``: every all-discrete model, and models with a
+continuous target or feature when a boosting option is set; the others use ``train.build_model``
+(scikit-learn).
 
 Boosting options (``model.lgb.boosting_type`` dart / goss / rf, ``reg_alpha``, ``min_split_gain``) run
 through ``dr_gbdt_train_ex``; at their defaults the trainer is called exactly as before."""
+import math
+
 import numpy as np
 
 from .forest import encoder_lut
@@ -25,45 +28,78 @@ def quant_bits(n_rows):
     return int(min(24, 30 - int(np.ceil(np.log2(max(n_rows, 2))))))
 
 
-def bin_sample(encoders, sample_codes, dict_sizes, max_bin=255):
+def bin_column(x, domain, max_real):
+    """One encoded feature -> (bins uint8 [n], n_bins, bin values).  x: the sample's float64 values (NaN =
+    NULL, which goes to the missing bin n_bins - 1); domain: the sorted distinct values the feature can
+    take (never NaN).  Up to max_real distinct values: one bin per value, bin values 1-D.  More: adjacent
+    values share a bin (LightGBM: max_bin = 255, train.py:106), bins of about equal sample counts, bin
+    values 2 x n_real (largest / smallest value of every bin); thresholds only fall between bins."""
+    ok = ~np.isnan(x)
+    pos = np.searchsorted(domain, x[ok])
+    if len(domain) > max_real:
+        cnt = np.bincount(pos, minlength=len(domain)).astype(np.float64)
+        edge = np.floor(np.cumsum(cnt) / max(cnt.sum(), 1.0) * max_real - 1e-9).astype(np.int64)
+        group = np.minimum(np.maximum.accumulate(np.clip(edge, 0, max_real - 1)), max_real - 1)
+        _, group = np.unique(group, return_inverse=True)      # dense bin ids, in value order
+        n_real = int(group.max()) + 1
+        values = np.stack([np.array([domain[group == b].max() for b in range(n_real)]),
+                           np.array([domain[group == b].min() for b in range(n_real)])])
+    else:
+        group, n_real, values = np.arange(len(domain)), len(domain), domain
+    out = np.full(len(x), n_real, dtype=np.uint8)                          # missing bin
+    out[ok] = group[pos].astype(np.uint8)
+    return out, n_real + 1, values
+
+
+def bin_sample(encoders, sample_codes, dict_sizes, max_bin=255, sample_values=None):
     """-> (bins uint8 [n, F'], n_bins int32 [F'], bin_values list of float arrays) or None.
-    A feature gets at most max_bin - 1 value bins (max_bin clamped to [2, 255]) plus the missing bin."""
+    A feature gets at most max_bin - 1 value bins (max_bin clamped to [2, 255]) plus the missing bin.
+    A discrete feature's domain is every value its encoder LUT holds; a continuous one ("cont" encoder,
+    float64 column of sample_values = {attr: values}, NaN = NULL) takes the sample's distinct values, +-inf
+    included, so an all-NULL column has only the missing bin and a single-valued one two bins.  None when
+    a continuous feature's values are not given or there are more than 128 encoded features."""
     max_real = min(255, max(2, int(max_bin))) - 1
     cols, n_bins, values = [], [], []
     for e in encoders:
         if e["type"] == "cont":
-            return None
-        lut = encoder_lut(e, dict_sizes[e["attr"]])
-        codes = np.asarray(sample_codes[e["attr"]], dtype=np.int64)
-        for j in range(lut.shape[1]):
-            col = lut[:, j]
-            vals = np.unique(col[~np.isnan(col)])
-            ok = ~np.isnan(col)
-            if len(vals) > max_real:
-                # more distinct values than bins (LightGBM: max_bin = 255, train.py:106): adjacent values
-                # share a bin, bins of about equal sample counts; thresholds only fall between bins
-                enc = col[codes + 1]
-                cnt = np.bincount(np.searchsorted(vals, enc[~np.isnan(enc)]), minlength=len(vals)).astype(np.float64)
-                edge = np.floor(np.cumsum(cnt) / max(cnt.sum(), 1.0) * max_real - 1e-9).astype(np.int64)
-                group = np.minimum(np.maximum.accumulate(np.clip(edge, 0, max_real - 1)), max_real - 1)
-                _, group = np.unique(group, return_inverse=True)      # dense bin ids, in value order
-                n_real = int(group.max()) + 1
-                upper = np.array([vals[group == b].max() for b in range(n_real)])
-                lower = np.array([vals[group == b].min() for b in range(n_real)])
-                bin_of = np.full(len(col), n_real, dtype=np.uint8)           # missing bin
-                bin_of[ok] = group[np.searchsorted(vals, col[ok])].astype(np.uint8)
-                cols.append(bin_of[codes + 1])
-                n_bins.append(n_real + 1)
-                values.append(np.stack([upper, lower]))
-                continue
-            bin_of = np.full(len(col), len(vals), dtype=np.uint8)           # missing bin
-            bin_of[ok] = np.searchsorted(vals, col[ok]).astype(np.uint8)
-            cols.append(bin_of[codes + 1])
-            n_bins.append(len(vals) + 1)
-            values.append(vals)
+            if sample_values is None or e["attr"] not in sample_values:
+                return None
+            x = np.asarray(sample_values[e["attr"]], dtype=np.float64)
+            parts = [bin_column(x, np.unique(x[~np.isnan(x)]), max_real)]
+        else:
+            lut = encoder_lut(e, dict_sizes[e["attr"]])
+            codes = np.asarray(sample_codes[e["attr"]], dtype=np.int64)
+            parts = [bin_column(lut[codes + 1, j], np.unique(lut[~np.isnan(lut[:, j]), j]), max_real)
+                     for j in range(lut.shape[1])]
+        for b, nb, v in parts:
+            cols.append(b)
+            n_bins.append(nb)
+            values.append(v)
     if not cols or len(cols) > 128:
         return None
     return np.stack(cols, axis=1).astype(np.uint8), np.asarray(n_bins, dtype=np.int32), values
+
+
+MIN_HESS_QUANTUM = 1024.0   # a regression row's quantised hessian: rounding bias <= 0.5 / 1024 of every leaf
+
+
+def regression_scale(y, init, n, goss_shift=0):
+    """-> k: a regression trains on y * 2^-k and its leaves and baseline are multiplied back by 2^k.
+    Every row's hessian 1 is quantised as the scale itself, 2^bits / max|y - init| / 2^goss_shift.  A spread
+    below 1 would push the hessian sums past int32; a large one (prices, incomes) rounds the hessian to a few
+    units or to 0, which biases every leaf or leaves the trees without a split.  So outside 1 <= spread with a
+    quantum >= MIN_HESS_QUANTUM, the target is brought to a spread in [1, 2), a quantum of at least
+    2^(bits - 1 - goss_shift).  Scaling by a power of two is exact, and with reg_alpha * 2^-k and min_split_gain
+    * 2^-2k every leaf of the scaled problem is the original's times 2^-k and every gain times 2^-2k in exact
+    arithmetic, so only the fineness of the quantisation changes.  Inside the window k = 0: the trainer runs
+    exactly as oracle/gbdt.py specifies it on the unscaled target."""
+    spread = float(np.abs(np.asarray(y, dtype=np.float64) - init).max())
+    if not spread > 0.0 or not np.isfinite(spread):
+        return 0
+    quantum = float(2 ** quant_bits(n)) / spread / float(1 << goss_shift)
+    if spread >= 1.0 and quantum >= MIN_HESS_QUANTUM:
+        return 0
+    return math.frexp(spread)[1] - 1          # spread = m * 2^e, m in [0.5, 1): spread * 2^-(e-1) in [1, 2)
 
 
 def class_weights(y_idx, n_classes, balanced):
@@ -150,21 +186,37 @@ def train_gpu(ctx, device, bins, n_bins, bin_values, y, n_classes, weight, n_ite
     from ._native import DR_GBDT_BOOST, dr_gbdt_boost, dr_gbdt_params
     if boosting not in DR_GBDT_BOOST:
         raise ValueError("boosting must be one of {}".format(sorted(DR_GBDT_BOOST)))
+    # the device indexes its shared-memory histograms with every bin byte: check them all before any launch
+    n_bins = np.asarray(n_bins, dtype=np.int32)
+    if bins.dtype != np.uint8 or bins.ndim != 2 or bins.shape[1] != len(n_bins):
+        raise ValueError("bins must be uint8 [n, {}] (one column per n_bins entry), got {} {}".format(
+            len(n_bins), bins.dtype, bins.shape))
+    if len(n_bins) and (int(n_bins.min()) < 1 or int(n_bins.max()) > 255):
+        raise ValueError("bins per feature must be in [1, 255]")
+    if bins.size and (bins >= n_bins).any():
+        f = int(np.flatnonzero((bins >= n_bins).any(axis=0))[0])
+        raise ValueError("feature {}: bin byte {} >= n_bins {}".format(f, int(bins[:, f].max()), int(n_bins[f])))
     n, F = bins.shape
     S = 1 if n_classes <= 2 else n_classes
+    top_k, other_k, goss_shift = goss_counts(n, top_rate, other_rate) if boosting == "goss" else (0, 0, 0)
+    k = 0
+    if n_classes == 1:
+        y = np.asarray(y, dtype=np.float64)
+        k = regression_scale(y, initial_scores(y, 1, None)[0], n, goss_shift)
+        y = np.ldexp(y, -k)
+        reg_alpha, min_split_gain = float(np.ldexp(reg_alpha, -k)), float(np.ldexp(min_split_gain, -2 * k))
     init = initial_scores(y, n_classes, weight)
     if n_classes == 1:
-        yv = np.asarray(y, dtype=np.float64)
-        qscale = float(2 ** quant_bits(n)) / max(float(np.abs(yv - init[0]).max()), 1e-300)
+        spread = float(np.abs(y - init[0]).max())
+        qscale = float(2 ** quant_bits(n)) / (spread if spread > 0.0 else 1.0)   # constant target: any scale
     else:
         qscale = float(2 ** quant_bits(n)) / float(np.max(weight))
     boost = None
     if boosting != "gbdt" or reg_alpha != 0.0 or min_split_gain != 0.0:
         boost = dr_gbdt_boost(DR_GBDT_BOOST[boosting], 0, 0, 0, float(reg_alpha), float(min_split_gain), None, None)
         if boosting == "goss":
-            top_k, other_k, shift = goss_counts(n, top_rate, other_rate)
             boost.goss_warmup, boost.goss_top_k, boost.goss_other_k = int(1.0 / learning_rate), top_k, other_k
-            qscale = qscale / float(1 << shift)
+            qscale = qscale / float(1 << goss_shift)
         if boosting == "dart":
             drop_off, drop_iter = dart_schedule(n_iter, learning_rate, seed, drop_rate, max_drop, skip_drop)
             boost.drop_off, boost.drop_iter = drop_off.ctypes.data, drop_iter.ctypes.data
@@ -186,7 +238,11 @@ def train_gpu(ctx, device, bins, n_bins, bin_values, y, n_classes, weight, n_ite
         ctx.gbdt_train_ex(prm, boost, d_bins, n_bins, d_yc, d_yv, d_w, init, ws, out_nodes, out_counts)
     nodes = out_nodes.cpu().numpy().view(NODE_DTYPE).reshape(n_iter, S, MAX_NODES)
     counts = out_counts.cpu().numpy().reshape(n_iter, S)
-    return flatten(nodes, counts, init, bin_values, F, n_classes)
+    forest = flatten(nodes, counts, init, bin_values, F, n_classes)
+    if k:                                    # back to the target's own units (exact)
+        forest["baseline"] = np.ldexp(forest["baseline"], k)
+        forest["value"] = np.ldexp(forest["value"], k)
+    return forest
 
 
 def flatten(nodes, counts, init, bin_values, n_features, n_classes):
@@ -210,7 +266,12 @@ def flatten(nodes, counts, init, bin_values, n_features, n_classes):
         tab_hi[f, :len(h)] = h
         tab_lo[f, :len(l)] = l
     fi, ti = np.where(leaf, 0, feat), flat["thr_bin"].astype(np.int64)
-    thr = np.where(leaf, 0.0, (tab_hi[fi, ti] + tab_lo[fi, np.minimum(ti + 1, max_bins)]) / 2.0)
+    hi, lo = tab_hi[fi, ti], tab_lo[fi, np.minimum(ti + 1, max_bins)]
+    with np.errstate(invalid="ignore", over="ignore"):
+        mid = (hi + lo) / 2.0
+    # +-inf neighbours, an overflowing sum or adjacent doubles (continuous features only): the split bin's
+    # largest value separates the two sides exactly as well
+    thr = np.where(leaf, 0.0, np.where(np.isfinite(mid) & (mid < lo), mid, hi))
     return {
         "n_features": int(n_features), "n_classes": int(n_classes), "baseline": np.asarray(init, dtype=np.float64),
         "tree_seq": np.tile(np.arange(S, dtype=np.int32), n_iter), "tree_offset": tree_offset,

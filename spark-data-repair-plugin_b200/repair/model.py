@@ -450,30 +450,64 @@ class RepairModel():
                           "current_value": pd.array(curs, dtype=object)})
 
 
-def _fit(rm, engine, encoders, codes, tile_col, features, dict_sizes, X, y_values, is_discrete, num_class, y=None):
-    """Model producer: the GPU histogram GBDT (gbdt.py) when every feature is discrete, else
-    scikit-learn's (train.py).  Both use the reference's fixed parameters (train.py:102-115) and the
-    tuned ones found by search.py (train.py:133-229: TPE-style search under k-fold CV, budget options
-    model.hp.* / model.cv.n_splits)."""
+def gpu_trainer_bins(trainer, opts, continuous, bin_fn):
+    """Which trainer _fit uses.  -> the GPU trainer's bins (gbdt.bin_sample's result) when dr_gbdt_train takes
+    the model, None when scikit-learn's histogram GBDT (train.build_model) does.
+    trainer: RepairModel.trainer; continuous: the model has a continuous target or feature; bin_fn() bins
+    the sample (None when it cannot be binned), called only when the options want the GPU trainer.
+    An all-discrete model goes to the GPU trainer; a continuous one only when model.lgb.boosting_type,
+    reg_alpha or min_split_gain is set, which scikit-learn has no counterpart for.  Either way the bins
+    must fit the trainer: at most 128 encoded features, 255 bins each, and the 200 KB histogram budget."""
+    from .train import _GPU_ONLY_OPTS, _get
+    if trainer == "sklearn":
+        return None
+    if continuous and all(_get(opts, k) == d for k, d in _GPU_ONLY_OPTS):
+        return None
+    binned = bin_fn()
+    if binned is None:
+        return None
+    n_bins = np.asarray(binned[1])
+    if len(n_bins) > 128 or int(n_bins.max()) > 255 or int(n_bins.sum()) * 12 > 200 * 1024:
+        return None
+    return binned
+
+
+def _fit(rm, engine, encoders, codes, vals, tile_col, cont_idx, features, dict_sizes, X, y_values, is_discrete,
+         num_class, y=None):
+    """Model producer: the GPU histogram GBDT (gbdt.py) or scikit-learn's (train.py), as gpu_trainer_bins
+    decides.  Both use the reference's fixed parameters (train.py:102-115) and the tuned ones found by
+    search.py (train.py:133-229: TPE-style search under k-fold CV, budget options model.hp.* /
+    model.cv.n_splits).  vals: the sample's float64 tile (columns cont_idx, NaN = NULL) or None."""
     from . import gbdt as G
     from . import search as HS
     from .train import _get, search_options
-    binned = None
     boosting = _get(rm.opts, "model.lgb.boosting_type")
-    if rm.trainer != "sklearn" and is_discrete:
-        binned = G.bin_sample(encoders, {f: codes[:, tile_col[f]] for f in features}, dict_sizes,
-                              max_bin=_get(rm.opts, "model.lgb.max_bin"))
-    if binned is not None and int(binned[1].sum()) * 12 <= 200 * 1024:
+    uses_cont = not is_discrete or any(e["type"] == "cont" for e in encoders)
+
+    def bin_fn():
+        if not is_discrete and not np.isfinite(y_values).all():
+            return None                  # no finite mean to start from: scikit-learn refuses it as well
+        return G.bin_sample(encoders, {f: codes[:, tile_col[f]] for f in features}, dict_sizes,
+                            max_bin=_get(rm.opts, "model.lgb.max_bin"),
+                            sample_values={f: vals[:, cont_idx[f]] for f in features if f in cont_idx}
+                            if vals is not None else None)
+
+    binned = gpu_trainer_bins(rm.trainer, rm.opts, uses_cont, bin_fn)
+    if binned is not None:
         bins, n_bins, values = binned
-        classes = sorted(set(int(v) for v in y_values.tolist()))
-        y_idx = np.searchsorted(np.asarray(classes), y_values).astype(np.int64)
+        if is_discrete:
+            classes = sorted(set(int(v) for v in y_values.tolist()))
+            y_fit = np.searchsorted(np.asarray(classes), y_values).astype(np.int64)
+        else:                            # regression: n_classes 1, unit weights, the mean as initial score
+            classes, y_fit = None, np.asarray(y_values, dtype=np.float64)
+        n_classes = len(classes) if is_discrete else 1
         balanced = _get(rm.opts, "model.lgb.class_weight") == "balanced"
         depth = _get(rm.opts, "model.lgb.max_depth")
 
         def train(params, rows=None):
-            b, yi = (bins, y_idx) if rows is None else (np.ascontiguousarray(bins[rows]), y_idx[rows])
-            w = G.class_weights(yi, len(classes), balanced)
-            return G.train_gpu(engine.ctx, engine.device, b, n_bins, values, yi, len(classes), w,
+            b, yi = (bins, y_fit) if rows is None else (np.ascontiguousarray(bins[rows]), y_fit[rows])
+            w = G.class_weights(yi, n_classes, balanced) if is_discrete else np.ones(len(yi))
+            return G.train_gpu(engine.ctx, engine.device, b, n_bins, values, yi, n_classes, w,
                                _get(rm.opts, "model.lgb.n_estimators"), _get(rm.opts, "model.lgb.learning_rate"),
                                depth if depth > 0 else 31,
                                num_leaves=int(min(max(params["num_leaves"], 2), 32)),   # the trainer's node budget
@@ -489,20 +523,26 @@ def _fit(rm, engine, encoders, codes, tile_col, features, dict_sizes, X, y_value
         defaults = HS.RF_DEFAULTS if boosting == "rf" else HS.DEFAULTS
         params = dict(defaults)
         if max_evals > 1 and y is not None:
-            folds = HS.cv_folds(y_idx, True, n_splits)
-            tile = engine.torch.from_numpy(np.ascontiguousarray(codes, dtype=np.int32)).to(engine.device)
+            folds = HS.cv_folds(y_fit, is_discrete, n_splits)
+            torch = engine.torch
+            tile = torch.from_numpy(np.ascontiguousarray(codes, dtype=np.int32)).to(engine.device)
             K = codes.shape[1]
+            # the float64 tile goes up once per model, and only for a model that reads or writes it
+            ctile = torch.from_numpy(np.ascontiguousarray(vals, dtype=np.float64)).to(engine.device) \
+                if uses_cont else None
+            n_cc = int(vals.shape[1]) if uses_cont else 0
+            out_col = tile_col[y] if is_discrete else cont_idx[y]
 
             def evaluate(p):
                 scores = []
                 for tr, va in folds:
                     spec = {"forest": train(p, tr), "encoders": encoders, "class_codes": classes, "integral": False}
-                    dm = DeviceModel(spec, tile_col, dict_sizes, {}, engine.device)
-                    work = tile.clone()
-                    cells = engine.torch.from_numpy(np.ascontiguousarray(va, dtype=np.int32)).to(engine.device)
-                    dm.predict(engine.ctx, work, K, None, 0, cells, len(va), tile_col[y])
-                    pred = work[cells.to(engine.torch.int64), tile_col[y]].cpu().numpy()
-                    scores.append(HS.score(y_values[va], pred, True))
+                    dm = DeviceModel(spec, tile_col, dict_sizes, cont_idx, engine.device)
+                    cells = torch.from_numpy(np.ascontiguousarray(va, dtype=np.int32)).to(engine.device)
+                    work, cwork = (tile.clone(), ctile) if is_discrete else (tile, ctile.clone())
+                    dm.predict(engine.ctx, work, K, cwork, n_cc, cells, len(va), out_col)
+                    pred = (work if is_discrete else cwork)[cells.to(torch.int64), out_col].cpu().numpy()
+                    scores.append(HS.score(y_values[va], pred, is_discrete))
                 return -float(np.mean(scores)), [-float(v) for v in scores]
 
             params, _, n_eval = HS.search(evaluate, max_evals, no_progress, timeout, defaults=defaults)
@@ -583,7 +623,8 @@ def _train_model(rm, engine, table, res, y, continuous, tile_col, fdeps=None):
     if rm.model_provider is not None:
         spec = rm.model_provider(ctx)
     else:
-        spec = _fit(rm, engine, encoders, codes, tile_col, features, dict_sizes, X, y_values, is_discrete, num_class, y)
+        spec = _fit(rm, engine, encoders, codes, vals, tile_col, cont_idx, features, dict_sizes, X, y_values,
+                    is_discrete, num_class, y)
     if spec is None:
         return ("const", None)
     if "const" in spec:
