@@ -588,6 +588,38 @@ int dr_null_bits(dr_ctx* ctx, const uint32_t* valid, int64_t bit_offset, int64_t
 int dr_flatten(dr_ctx* ctx, const int32_t* const* cols, const int64_t* base, int n_cols, int64_t n_rows,
                const int64_t* row_ids, int32_t* out_codes, uint32_t* out_valid, int64_t* out_ids, void* stream);
 
+/* ---- Spark-compatible distinct counts (opt-in; RepairApi.scala:108-118 computeColumnStats, :430-437
+ * approx_count_distinct(struct(x, y))) ----------------------------------------------------------------
+ * HyperLogLog++ registers as Spark builds them with relative SD 0.05 (p = 9): x = XxHash64(value, seed 42),
+ * register x >> 55 keeps the max of nlz((x << 9) | (1 << 8)) + 1.  `regs` is device int32[512], zeroed by
+ * the caller and updated with atomicMax (so calls accumulate).  The estimate is computed on the host.
+ * Value kinds: DR_HLL_STRING = UTF-8 bytes, Arrow layout (data: 8-byte aligned device bytes, offsets: device
+ * int64[n + 1]); DR_HLL_INT / DR_HLL_LONG = device int32 / int64 values (byte, short, boolean 0/1 travel as
+ * int32); DR_HLL_FLOAT / DR_HLL_DOUBLE = device float / double, hashed through their bits after -0.0 -> 0.0
+ * and NaN -> the canonical NaN.
+ * dr_hll_dict: registers of the n dictionary entries; hashes (device uint64[n], may be NULL) receives every
+ *   entry's hash (the seeds of a pair's struct hash).
+ * dr_hll_pairs: for each pair, registers of struct(x, y) over its presence bits (device uint32 words, bit
+ *   i * (dom_y + 1) + j set iff x slot i occurs with y slot j; slot 0 = NULL, slot c + 1 = code c): the hash
+ *   of bit (i, j) is XxHash64(y entry j - 1, seed = hx[i - 1]), where a NULL slot passes the seed through
+ *   (x NULL: seed 42; y NULL: the hash is the seed). */
+#define DR_HLL_STRING 0
+#define DR_HLL_INT 1
+#define DR_HLL_LONG 2
+#define DR_HLL_FLOAT 3
+#define DR_HLL_DOUBLE 4
+typedef struct {
+    const uint64_t* hx;   /* device uint64[dom_x]: seed 42 hash of each x code */
+    const void* y_data;   /* y entries, as dr_hll_dict takes them */
+    const int64_t* y_off; /* DR_HLL_STRING only */
+    const uint32_t* bits; /* the pair's presence words */
+    int32_t* regs;        /* device int32[512] */
+    int32_t dom_x, dom_y, y_kind;
+} dr_hll_pair;
+int dr_hll_dict(dr_ctx* ctx, int32_t kind, const void* data, const int64_t* offsets, int64_t n, uint64_t* hashes,
+                int32_t* regs, void* stream);
+int dr_hll_pairs(dr_ctx* ctx, const dr_hll_pair* pairs, int n_pairs, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -68,6 +68,15 @@ class dr_gbdt_boost(ctypes.Structure):
 DR_GBDT_BOOST = {"gbdt": 0, "dart": 1, "goss": 2, "rf": 3}
 
 
+class dr_hll_pair(ctypes.Structure):
+    _fields_ = [("hx", c_void_p), ("y_data", c_void_p), ("y_off", c_void_p), ("bits", c_void_p), ("regs", c_void_p),
+                ("dom_x", c_int32), ("dom_y", c_int32), ("y_kind", c_int32)]
+
+
+# value kinds of dr_hll_dict / dr_hll_pairs by Spark type (byte / short / boolean travel as int32)
+DR_HLL_KIND = {"string": 0, "int": 1, "boolean": 1, "long": 2, "float": 3, "double": 4}
+
+
 # ---- argument kinds --------------------------------------------------------------------------------
 # Pointer-width ctypes types whose from_param converts a Python value at call time.  ctypes keeps what
 # from_param returns alive until the C function returns, so the host arrays built here need no other
@@ -197,6 +206,8 @@ _SIGNATURES = {
     "dr_error_map": (c_int, [c_void_p, _Bufs, c_int, c_int64, _Buf, c_void_p]),
     "dr_null_bits": (c_int, [c_void_p, _Buf, c_int64, c_int64, c_int64, c_uint64, c_double, _Buf, c_void_p]),
     "dr_flatten": (c_int, [c_void_p, _Bufs, _I64s, c_int, c_int64, _Buf, _Buf, _Buf, _Buf, c_void_p]),
+    "dr_hll_dict": (c_int, [c_void_p, c_int32, _Buf, _Buf, c_int64, _Buf, _Buf, c_void_p]),
+    "dr_hll_pairs": (c_int, [c_void_p, POINTER(dr_hll_pair), c_int, c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(sorted(_SIGNATURES))
@@ -538,6 +549,21 @@ class Context:
 
     def flatten(self, cols, base, n_rows, row_ids, out_codes, out_valid, out_ids):
         self._call("dr_flatten", cols, base, len(cols), n_rows, row_ids, out_codes, out_valid, out_ids)
+
+    # ---- Spark-compatible distinct counts ---------------------------------------------------------------
+    def hll_dict(self, kind, data, offsets, n, regs, hashes=None):
+        """regs (device int32[512]) <- HLL++ registers of n dictionary entries; hashes (device uint64[n])
+        receives each entry's seed-42 hash when given."""
+        self._call("dr_hll_dict", kind, data, offsets, n, hashes, regs)
+
+    def hll_pairs(self, pairs):
+        """pairs: [(hx, y_kind, y_data, y_off, dom_x, dom_y, bits, regs)], buffers as tensors or addresses."""
+        arr = (dr_hll_pair * max(len(pairs), 1))()
+        for d, (hx, y_kind, y_data, y_off, dom_x, dom_y, bits, regs) in zip(arr, pairs):
+            d.hx, d.y_data, d.y_off = _address(hx), _address(y_data), _address(y_off)
+            d.bits, d.regs = _address(bits), _address(regs)
+            d.dom_x, d.dom_y, d.y_kind = dom_x, dom_y, y_kind
+        self._call("dr_hll_pairs", arr, len(pairs))
 
 
 def _profiled(name, fn):

@@ -14,6 +14,7 @@ import time
 import numpy as np
 
 from . import constraints as DC
+from . import hll as HLL
 from . import stats_host as SH
 from ._native import DR_OP, Context
 from .table import DeviceTable
@@ -173,6 +174,8 @@ class Engine:
         self.disc_dom = {}       # attr -> domain size of that column
         self.timings = {}
         self.trace = None        # list of (label, seconds since the previous mark) when tracing
+        self.spark_ndv = False   # distinct counts as Spark's HyperLogLog++ estimates them (repair/hll.py)
+        self.ndv_provenance = {}  # spark_ndv: {"columns": {attr: how}, "pairs": {(x, y): how}}, how = estimate | exact
 
     # ------------------------------------------------------------------------------------------
     @property
@@ -224,23 +227,29 @@ class Engine:
 
     # ---- a7: discretisation ------------------------------------------------------------------
     def discretize(self, discrete_thres):
-        """convertToDiscretizedTable (RepairApi.scala:126-169) -> domain_stats; fills disc_cols."""
+        """convertToDiscretizedTable (RepairApi.scala:126-169) -> domain_stats; fills disc_cols.  With spark_ndv
+        the domain sizes and the keep decision come from the HyperLogLog++ estimates; the discretised domains
+        (disc_dom) stay the exact dictionary sizes either way."""
         assert 2 <= discrete_thres < 65536
         domain_stats = {}
         self.disc_cols, self.disc_dom = {}, {}
+        counts = {}
+        if self.spark_ndv:
+            counts = HLL.column_counts(self.ctx, self.device, self.table.columns)
+            self.ndv_provenance = {"columns": {a: how for a, (_, how) in counts.items()}, "pairs": {}}
         for c in self.table.columns:
-            ndv = c.dict_size
+            ndv = counts[c.name][0] if self.spark_ndv else c.dict_size
             domain_stats[c.name] = ndv
             if c.continuous:
                 out = self.torch.full((self.dt.n_pad,), -1, dtype=self.torch.int32, device=self.device)
-                if ndv > 0:
+                if c.dict_size > 0:
                     vmin, den = SH.discretize_params(c.kind, c.dictionary[0], c.dictionary[-1])
                     self.ctx.discretize(self.dt.val(c.name), self.n_rows, vmin, den, discrete_thres, out)
                 self.disc_cols[c.name] = out
                 self.disc_dom[c.name] = discrete_thres + 1
             elif 1 < ndv <= discrete_thres:
                 self.disc_cols[c.name] = self.dt.col(c.name)
-                self.disc_dom[c.name] = ndv
+                self.disc_dom[c.name] = c.dict_size
             else:
                 _logger.warning("'{}' dropped because of its unsuitable domain (size={})".format(c.name, ndv))
         return domain_stats
@@ -830,6 +839,48 @@ class Engine:
             nnz.update(got)
         return tables, nnz
 
+    def _disc_hash_values(self, a):
+        """The values of discretised attribute `a` as Spark hashes them, in code order: a kept column's dictionary,
+        the int buckets 0 .. thres of a continuous one -> (kind, device data, device offsets, n)."""
+        col = self.table.by_name[a]
+        if col.continuous:
+            return HLL.value_buffers(a, np.arange(self.disc_dom[a]), "int", self.device)
+        return HLL.value_buffers(a, col.dictionary, HLL.spark_type(col), self.device)
+
+    def pair_distinct_counts(self, pairs):
+        """approx_count_distinct(struct(x, y)) as Spark estimates it, for ordered pairs of discretised attributes:
+        full-table presence bits (OR-combined across the shards), then dr_hll_pairs over them.  Pairs that
+        reference more than 64 attributes take several presence launches.
+        -> ({(x, y): count}, presence map of the pairs, or None when they took several launches)"""
+        torch = self.torch
+        batches, attrs = [[]], set()
+        for p in pairs:
+            if batches[-1] and len(attrs | set(p)) > 64:
+                batches.append([])
+                attrs = set()
+            batches[-1].append(p)
+            attrs |= set(p)
+        vals, hx = {}, {}
+        for a in dict.fromkeys(a for p in pairs for a in p):
+            vals[a] = self._disc_hash_values(a)
+            kind, data, off, n = vals[a]
+            hx[a] = torch.empty(max(n, 1), dtype=torch.uint64, device=self.device)
+            self.ctx.hll_dict(kind, data, off, n, torch.zeros(HLL.M, dtype=torch.int32, device=self.device), hx[a])
+        counts, present = {}, None
+        for batch in batches:
+            launched = self.launch_pair_presence(batch, full=True)
+            self.exchange([(launched[2], "or")])
+            nnz, present, _ = self.pair_presence_host(launched, check_cover=False)
+            _, offs, bits, _ = launched
+            regs = torch.zeros((len(batch), HLL.M), dtype=torch.int32, device=self.device)
+            self.ctx.hll_pairs([(hx[x], vals[y][0], vals[y][1], vals[y][2], self.disc_dom[x], self.disc_dom[y],
+                                 bits.data_ptr() + 4 * offs[q], regs[q]) for q, (x, y) in enumerate(batch)])
+            regs_h = regs.cpu().numpy()
+            for q, p in enumerate(batch):
+                counts[p], how = HLL.distinct_count(regs_h[q], nnz[frozenset(p)])
+                self.ndv_provenance.setdefault("pairs", {})[p] = how
+        return counts, (present if len(batches) == 1 else None)
+
     def compute_attr_stats(self, targets, domain_stats, attr_freq_thr, pairwise_thr, max_attrs, presence=None):
         """computeAttrStats (RepairApi.scala:396-477) -> (pairwise_stats, tables, having).
         presence: (nnz lower bounds, presence matrices, exact) of a pair sample that was already taken
@@ -849,7 +900,12 @@ class Engine:
 
         selected = {t: list(cands[t]) for t in targets if t not in scoring}
         tables, present = {}, None
-        if scoring:
+        if scoring and self.spark_ndv:
+            est, present = self.pair_distinct_counts(list(dict.fromkeys(p for t in scoring for p in cands[t])))
+            for t in scoring:
+                selected[t] = SH.select_scored(cands[t], {frozenset(p): est[p] for p in cands[t]}, domain_stats,
+                                               pairwise_thr, max_attrs)
+        elif scoring:
             all_scored = uniq([p for t in scoring for p in cands[t]])
             if presence is not None and all(frozenset(p) in presence[0] for p in all_scored):
                 lower, present, exact = presence
@@ -1029,7 +1085,9 @@ class Engine:
                     if frozenset(pr) not in seen:
                         seen.add(frozenset(pr))
                         scored.append(pr)
-        pres_launched = self.launch_pair_presence(scored) if scored and len(res.disc_attrs) <= 64 else None
+        # (spark_ndv: the scored pairs take full-table presence bits in compute_attr_stats instead)
+        pres_launched = self.launch_pair_presence(scored) if scored and not self.spark_ndv and \
+            len(res.disc_attrs) <= 64 else None
         self.mark("detect:local 1 launched")
         # (sharded: "did the presence sample cover every shard completely" rides in the same collective)
         cover = None

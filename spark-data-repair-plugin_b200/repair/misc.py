@@ -137,8 +137,14 @@ class RepairMisc():
         CAST(.. AS STRING) of numeric extremes; ``avgLen`` / ``maxLen`` are the ceiling of the mean and the
         maximum character length of strings (20, Spark's defaultSize, for an all-NULL string column) and the
         source type's size for numbers; ``hist`` (numbers only) are the gaps between the percentiles at
-        i / num_bins (the ceil(p n)-th smallest value) normalised by their sum.  One dr_scan_hist pass."""
+        i / num_bins (the ceil(p n)-th smallest value) normalised by their sum.  One dr_scan_hist pass.
+        Option ``spark_compatible_distinct_counts`` ("true" / "false", default "false"): ``distinctCnt`` is
+        Spark's HyperLogLog++ estimate (repair/hll.py; the exact count inside the bias-table band)."""
         self._check_required_options(["table_name"])
+        spark_ndv = self.opts.get("spark_compatible_distinct_counts", "false").strip().lower()
+        if spark_ndv not in ("true", "false"):
+            raise ValueError("Option 'spark_compatible_distinct_counts' must be 'true' or 'false', but '{}' "
+                             "found".format(self.opts["spark_compatible_distinct_counts"]))
         num_bins = 8
         if "num_bins" in self.opts:
             try:
@@ -151,6 +157,14 @@ class RepairMisc():
         tbl, _, _ = self._load()
         cols = encode_columns(tbl)
         hists = _device_hists(cols)
+        ndv = {}
+        if spark_ndv == "true":
+            from . import hll as HLL
+            ctx, device = _acquire()
+            try:
+                ndv = HLL.column_counts(ctx, device, cols)
+            finally:
+                _release(ctx)
         rows = []
         for col, h in zip(cols, hists):
             cnt = h[1:]
@@ -170,7 +184,8 @@ class RepairMisc():
                     max_len = int(lens[present].max())
                 else:
                     avg_len = max_len = col.default_size
-            rows.append((col.name, int(len(present)), mn, mx, int(h[0]), int(avg_len), int(max_len), hist))
+            distinct = ndv[col.name][0] if ndv else int(len(present))
+            rows.append((col.name, distinct, mn, mx, int(h[0]), int(avg_len), int(max_len), hist))
         names = ["attrName", "distinctCnt", "min", "max", "nullCnt", "avgLen", "maxLen", "hist"]
         return pd.DataFrame({c: pd.Series([r[i] for r in rows], dtype=object if c in ("attrName", "min", "max", "hist")
                                            else np.int64) for i, c in enumerate(names)})

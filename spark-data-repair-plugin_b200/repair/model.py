@@ -109,6 +109,7 @@ class RepairModel():
         self.distributed = None      # torch.distributed process group (or True = default group): row-sharded run
         self.frozen_models = None    # models of an earlier run() (setFrozenModels): skips the training phase
         self.borrow_encoded_output = False   # encoded result arrays may alias a reusable pinned buffer (bench loop)
+        self.spark_compatible_distinct_counts = False   # HyperLogLog++ estimates as Spark computes them (repair/hll.py)
         self.last_run: Dict[str, Any] = {}
 
     # ---- setters (same names / checks / messages as the reference) -------------------------------
@@ -150,6 +151,19 @@ class RepairModel():
         training again: inference-only passes over new batches of the same table (same columns and
         dictionaries).  The reference retrains on every run (model.py:1001-1052); not part of its API."""
         self.frozen_models = models
+        return self
+
+    @argtype_check
+    def setSparkCompatibleDistinctCounts(self, enabled: bool) -> "RepairModel":
+        """Take every distinct count that drives a decision -- the domain sizes of the discretisation
+        (``domain_stats``), the attribute-pair scores and what reads them (domain-analysis thresholds,
+        entropies, encoder choice, rule domain limit) -- from Spark's HyperLogLog++ estimates (relative SD
+        0.05) instead of exact counts, so that a run makes the reference's choices.  Inside the band where
+        Spark corrects the estimate with the HLL++ paper's bias tables (roughly 400 - 2600 distinct values)
+        the exact count is used; ``last_run["distinct_count_provenance"]`` tells which is which.  Numeric
+        columns hash by their source dtype: pass a column that Spark read as IntegerType as int32.  Off by
+        default; not part of the reference API."""
+        self.spark_compatible_distinct_counts = enabled
         return self
 
     def setEncodedInput(self, table: EncodedTable) -> "RepairModel":
@@ -342,6 +356,7 @@ class RepairModel():
             dist = Dist(None if self.distributed is True else self.distributed)
             table = table.unify(dist, dt, ctx)
         engine = Engine(table, self.device_index, dist=dist, device_table=dt, ctx=ctx)
+        engine.spark_ndv = bool(self.spark_compatible_distinct_counts)
         ingest["engine_ready_s"] = time.time() - t0
         try:
             detectors = self.error_detectors or default_detectors(self.targets, table.names)
@@ -350,6 +365,8 @@ class RepairModel():
                                 self._given_cells(table))
             self.last_run = {"detect": res, "elapsed_detect": time.time() - t0}
             self.last_run.update(ingest)
+            if engine.spark_ndv:
+                self._record_provenance(engine.ndv_provenance)
             self.last_run["detect_done_s"] = time.time() - t0
             if detect_errors_only:
                 return _maybe_arrow(self._cells_frame(engine, table, res), arrow_io)
@@ -380,6 +397,14 @@ class RepairModel():
             self.last_run["gpu_launches"] = engine.launches + (engine._launches0 - launches0 if ctx is not None else 0)
             engine.close()
             self.last_run["total_s"] = time.time() - t0
+
+    def _record_provenance(self, prov):
+        self.last_run["distinct_count_provenance"] = prov
+        cols = [a for a, how in prov.get("columns", {}).items() if how != "estimate"]
+        pairs = ["({}, {})".format(x, y) for (x, y), how in prov.get("pairs", {}).items() if how != "estimate"]
+        if cols or pairs:
+            _logger.warning("Spark-compatible distinct counts: exact counts used inside the HyperLogLog++ bias-table "
+                            "band for columns [{}] and pairs [{}]".format(", ".join(cols), ", ".join(pairs)))
 
     # ---- pmf / score / maximal-likelihood modes (model.py:1350-1390) -------------------------------
     def _run_pmf_modes(self, engine, table, res, continuous, compute_repair_prob, compute_repair_score,

@@ -15,10 +15,13 @@ ROW_ALIGN = 128  # rows are padded so that every column starts 512-byte aligned 
 class Column:
     """kind: 'str' (discrete) | 'int' | 'float' (both continuous, RepairBase.scala:41-44).
     ``dictionary``: sorted distinct non-NULL values (str objects, or float64 for numerics);
-    ``codes``: int32 index into it, -1 = NULL;  ``values``: float64 (NaN = NULL) for numerics."""
+    ``codes``: int32 index into it, -1 = NULL;  ``values``: float64 (NaN = NULL) for numerics.
+    ``spark_type``: the Spark type of the source column ('string', 'int', 'long', 'float', 'double',
+    'boolean'), or None when unknown; only the Spark-compatible distinct counts (repair/hll.py) read it."""
 
-    def __init__(self, name, kind, dictionary, codes, values=None):
+    def __init__(self, name, kind, dictionary, codes, values=None, spark_type=None):
         self.name, self.kind, self.dictionary, self.values = name, kind, dictionary, values
+        self.spark_type = spark_type
         self._codes = codes      # host int32 array, or a callable that fetches it (device-resident ingest)
 
     @property
@@ -76,13 +79,35 @@ class Column:
         return [None if c < 0 else strs[c] for c in np.asarray(codes).tolist()]
 
 
-def _encode_numeric(name, kind, arr):
+def _encode_numeric(name, kind, arr, spark_type=None):
     vals = np.asarray(arr, dtype=np.float64)
     nul = np.isnan(vals)
     uniq = np.unique(vals[~nul])
     codes = np.full(len(vals), -1, dtype=np.int32)
     codes[~nul] = np.searchsorted(uniq, vals[~nul]).astype(np.int32)
-    return Column(name, kind, uniq, codes, vals)
+    return Column(name, kind, uniq, codes, vals, spark_type)
+
+
+def _numpy_spark_type(dtype, kind):
+    """Spark type of a numeric numpy / pandas dtype (int8 / int16 / int32 -> int, int64 -> long, float32 -> float,
+    float64 -> double); columns of Python objects take the widest type of their kind."""
+    k, size = getattr(dtype, "kind", "O"), int(getattr(dtype, "itemsize", 8))
+    if k in "iu":
+        return "int" if size < 4 or (k == "i" and size == 4) else "long"
+    if k == "f":
+        return "float" if size <= 4 else "double"
+    return "long" if kind == "int" else "double"
+
+
+def _arrow_spark_type(t):
+    import pyarrow as pa
+    if pa.types.is_boolean(t):
+        return "boolean"
+    if pa.types.is_integer(t):
+        return "int" if t.bit_width < 32 or (t.bit_width == 32 and pa.types.is_signed_integer(t)) else "long"
+    if pa.types.is_floating(t):
+        return "float" if t.bit_width <= 32 else "double"
+    return "string"
 
 
 def _encode_arrow_strings(name, arr):
@@ -101,7 +126,7 @@ def _encode_arrow_strings(name, arr):
     used[raw[valid]] = True
     dictionary, lut = _sorted_dictionary(entries, used)
     codes = np.where(valid, lut[raw], -1).astype(np.int32) if len(entries) else np.full(len(raw), -1, dtype=np.int32)
-    return Column(name, "str", dictionary, codes, None)
+    return Column(name, "str", dictionary, codes, None, "string")
 
 
 def _encode_strings(name, series):
@@ -125,7 +150,7 @@ def _encode_strings(name, series):
     codes = np.full(len(strs), -1, dtype=np.int32)
     if len(present):
         codes[~isn] = np.fromiter((lut[v] for v in present.tolist()), dtype=np.int32, count=len(present))
-    return Column(name, "str", uniq, codes, None)
+    return Column(name, "str", uniq, codes, None, "string")
 
 
 def _arrow_gate(tbl, row_id, name):
@@ -204,11 +229,13 @@ def encode_columns(tbl):
                     kind = "float"
             if kind is not None:
                 arr = pd.to_numeric(s, errors="coerce").to_numpy(dtype=np.float64, na_value=np.nan)
-                col = _encode_numeric(str(c), kind, arr)
+                col = _encode_numeric(str(c), kind, arr, _numpy_spark_type(s.dtype, kind))
             else:
                 if k == "b":
                     s = s.map(lambda v: None if v is None or v != v else ("true" if v else "false"))
                 col = _encode_strings(str(c), s)
+                if k == "b":
+                    col.spark_type = "boolean"
                 size = STRING_DEFAULT_SIZE
             col.default_size = size
             cols.append(col)
@@ -224,12 +251,13 @@ def encode_columns(tbl):
             if pa.types.is_dictionary(arr.type):
                 arr = arr.dictionary_decode()
             vals = np.asarray(pc.cast(arr, pa.float64()).to_numpy(zero_copy_only=False), dtype=np.float64)
-            col = _encode_numeric(f.name, "int" if pa.types.is_integer(t) else "float", vals)
+            col = _encode_numeric(f.name, "int" if pa.types.is_integer(t) else "float", vals, _arrow_spark_type(t))
             col.default_size = t.bit_width // 8
         else:
             if not (pa.types.is_string(t) or pa.types.is_large_string(t)):
                 arr = pc.cast(arr.dictionary_decode() if pa.types.is_dictionary(arr.type) else arr, pa.string())
             col = _encode_arrow_strings(f.name, arr)
+            col.spark_type = _arrow_spark_type(t)
             col.default_size = STRING_DEFAULT_SIZE
         cols.append(col)
     return cols
@@ -316,7 +344,7 @@ class EncodedTable:
                 cols.append(_encode_strings(c, df[c]))
             else:
                 arr = pd.to_numeric(df[c], errors="coerce").to_numpy(dtype=np.float64, na_value=np.nan)
-                cols.append(_encode_numeric(c, kinds[c], arr))
+                cols.append(_encode_numeric(c, kinds[c], arr, _numpy_spark_type(df[c].dtype, kinds[c])))
         return cls(row_id, df[row_id].to_numpy(), kinds[row_id], cols, name)
 
     @classmethod
@@ -348,7 +376,9 @@ class EncodedTable:
                 if pa.types.is_dictionary(arr.type):
                     arr = arr.dictionary_decode()
                 vals = pc.cast(arr, pa.float64()).to_numpy(zero_copy_only=False)
-                cols.append(_encode_numeric(f.name, kinds[f.name], np.asarray(vals, dtype=np.float64)))
+                cols.append(_encode_numeric(f.name, kinds[f.name], np.asarray(vals, dtype=np.float64),
+                                            _arrow_spark_type(f.type.value_type if pa.types.is_dictionary(f.type)
+                                                              else f.type)))
                 continue
             cols.append(_encode_arrow_strings(f.name, arr))
         ids = plain(tbl[row_id])
@@ -468,7 +498,7 @@ class EncodedTable:
                 dictionary, lut = _sorted_dictionary(entries, bits.astype(bool))
                 luts.append(lut)
                 loff.append(loff[-1] + len(lut))
-                table_cols[i] = Column(attrs[i], "str", dictionary, None, None)
+                table_cols[i] = Column(attrs[i], "str", dictionary, None, None, "string")
             phases["sort_dictionaries_s"] += time.perf_counter() - t_w
             t_w = time.perf_counter()
             with torch.cuda.stream(side):
@@ -613,7 +643,8 @@ class EncodedTable:
             else:
                 codes = np.where(c.codes >= 0, np.r_[lut, np.int32(-1)][c.codes], -1).astype(np.int32) if len(lut) else \
                     np.full(len(c.codes), -1, dtype=np.int32)
-            cols.append(Column(c.name, kind, merged, codes, values))
+            cols.append(Column(c.name, kind, merged, codes, values,
+                               c.spark_type if len(kinds) == 1 else None))
         t = EncodedTable(self.row_id, self._row_ids, self.row_id_kind, cols, self.name, n_rows=self.n_rows)
         t.row_offset = int(sum(counts[:dist.rank]))
         t.n_rows_global = int(sum(counts))
@@ -625,8 +656,8 @@ class EncodedTable:
         """Contiguous row shard [lo, hi) for rank `rank` of `world` (global dictionaries kept)."""
         n = self.n_rows
         lo, hi = (n * rank) // world, (n * (rank + 1)) // world
-        cols = [Column(c.name, c.kind, c.dictionary, c.codes[lo:hi], None if c.values is None else c.values[lo:hi])
-                for c in self.columns]
+        cols = [Column(c.name, c.kind, c.dictionary, c.codes[lo:hi], None if c.values is None else c.values[lo:hi],
+                       c.spark_type) for c in self.columns]
         t = EncodedTable(self.row_id, self.row_ids[lo:hi], self.row_id_kind, cols, self.name)
         t.row_offset, t.n_rows_global = lo, n
         return t
